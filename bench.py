@@ -18,7 +18,14 @@ Frames are synthetic "S-photo" images (SURVEY.md section 8d), one distinct frame
             -- H2D/D2H and the host codestream writer/reader inside the timed region.  `e2e.pipelined_*` is the same
             loop from several host threads / coder pairs / streams (PCIe full duplex), reported beside it.
   roofline: for the slowest GPU stage: algorithmic bytes of SURVEY.md section 8d (9 B/pixel for the
-            transform kernels, 6+c for the Huffman kernels) / its CUDA-event time / measured HBM peak.
+            transform kernels, 6+c for the Huffman kernels) / its CUDA-event time / HBM peak (MEASURED_PEAKS.json
+            when present, else the H100 SXM data-sheet 3.35 TB/s).
+  device  : the GPU's name and power limit, read in the same run: a number is only worth something with them.
+
+  --dump-outputs DIR: after the timed steps, what the timed path computed in its last step is written as DIR/<name>.npy
+            (float32; an array of more than DUMP_CAP values is sampled at seeded positions): the JPEG bytes and the
+            quantised coefficients of the encoder and the decoded pixels, so that two builds can be compared output for
+            output on the same inputs.  Not with --impl reference.
   cpu_baseline / --impl reference : the CPU oracle (oracle/liboracle.so, a port of the reference's CPU
             path, byte-identical to the reference's own gpujpeg_huffman_cpu_* code) on all host cores.
 """
@@ -43,11 +50,39 @@ def hbm_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
+
+
+def device_line(index):
+    """name and power limit of the GPU the numbers were measured on"""
+    import torch
+    out = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=20).stdout.strip()
+        out["power_limit_w"] = float(q)
+    except Exception:
+        pass
+    return out
+
+
+DUMP_CAP = 4 << 20   # values written per array: 16 MB as float32, three sampled arrays at most
+
+
+def dump_outputs(out_dir, arrays):
+    """each array as <out_dir>/<name>.npy in float32 (exact for the u8 pixels and i16 coefficients): whole when it has at
+    most DUMP_CAP values, else DUMP_CAP of them at sorted positions drawn from a fixed seed (the same for the same size)"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        flat = np.asarray(a).reshape(-1)
+        if flat.size > DUMP_CAP:
+            flat = flat[np.sort(np.random.default_rng(0).integers(0, flat.size, DUMP_CAP))]
+        np.save(os.path.join(out_dir, name + ".npy"), flat.astype(np.float64 if flat.dtype == np.float64 else np.float32))
 
 
 class ClockSampler:
-    """SM clock + throttle reasons sampled DURING the timed regions (B200_PROFILING.md clocks line).  NVML in a thread
+    """SM clock + throttle reasons sampled DURING the timed regions.  NVML in a thread
     of this process (the counters nvidia-smi prints; ~2 ms period, so even a 10 ms timed region is covered);
     falls back to an `nvidia-smi -lms` child when the NVML binding is missing."""
 
@@ -176,7 +211,7 @@ def cpu_frames(width, height, rst, frames, threads):
 
 def reference_gpu(kind, width, height, rst, iters=10):
     """'The kernel to beat': the reference's own GPU library (compiled in place into oracle/_ref by `make -C oracle refgpu`,
-    its CUDA kernels recompiled for sm_100) on the same box, same frame, pinned host buffers obtained through its own
+    its CUDA kernels compiled for sm_90a) on the same box, same frame, pinned host buffers obtained through its own
     gpujpeg_image_load_from_file, serial calls, perf_stats on -- in a child process, so that its gpujpeg_* symbols never
     meet the product's.  An extra of the record, not part of any timed region of this benchmark."""
     so = os.path.join(ROOT, "oracle", "_ref", "libgpujpeg_refgpu.so")
@@ -344,6 +379,8 @@ def run_batch(args, g, o, torch, dist, rank, world, local, dev, numa, nccl_log):
         step_resident()
     ms = timed(step_resident, args.steps)
     value = n_frames * npix / (ms * 1e-3) / 1e6
+    if args.dump_outputs and rank == 0:   # the last frame this rank decoded, and every stream's size
+        dump_outputs(args.dump_outputs, {"decoded_rgb_last_frame": d_out.cpu().numpy(), "jpeg_sizes": np.array(sizes)})
 
     scattered = None
     if world > 1:
@@ -378,7 +415,7 @@ def run_batch(args, g, o, torch, dist, rank, world, local, dev, numa, nccl_log):
                        "sharding": "frames round-robin over ranks, no data-path collective; `scattered`: NCCL send/recv of raw "
                                    "frames from rank 0 + gather-v of the streams"},
             "scattered": scattered, "jpeg_bytes_per_frame": int(np.mean(sizes)) if sizes else None,
-            "gpu_launches": 6 * len(mine) * args.steps, "clocks": clocks, "numa": numa})
+            "gpu_launches": 6 * len(mine) * args.steps, "clocks": clocks, "numa": numa, "device": device_line(local)})
     enc.close()
     dec.close()
     if world > 1:
@@ -428,9 +465,12 @@ def main():
     # BASELINE.json config 5: a fixed batch of frames sharded round-robin over the ranks (strong scaling); with --batch the
     # step is the whole batch.  `--size 16k --batch 32` is the configuration the reference's north star names.
     ap.add_argument("--batch", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes what the GPU path computed; --impl reference has no such output")
         return run_reference(args)
 
     import numpy as np
@@ -510,6 +550,12 @@ def main():
     ms_total = timed(step_resident, args.steps)
     ms_step = ms_total / args.steps
     value = world * npix / (ms_step * 1e-3) / 1e6
+    if args.dump_outputs and rank == 0:   # the last timed step: the encoder's JPEG bytes and coefficients, K4's pixels
+        last = enc.stream()
+        assert np.array_equal(last, jpeg), "the timed encode produced other bytes than the first call"
+        dump_outputs(args.dump_outputs, {"jpeg_bytes": last, "jpeg_size": np.array([last.size], np.float64),
+                                         "coefficients": enc.coefficients(width, height, (lh, lv), args.interleaved),
+                                         "decoded_rgb": d_out.cpu().numpy()})
 
     # ---- per-stage times for the roofline (same stream, CUDA events, inputs > L2) ----
     stages = {}
@@ -610,19 +656,6 @@ def main():
         alg = {"k1_fdct": 3.0 + coef_bpp, "k2_huffman_encode": coef_bpp + c_bpp, "k3_huffman_decode": coef_bpp + c_bpp,
                "k4_idct": 3.0 + coef_bpp, "k0_marker_scan": 2.0 * c_bpp}
         worst = max((k for k in stages if k != "k0_marker_scan"), key=lambda k: stages[k])
-        # DRAM traffic of that kernel from the committed ncu --set full capture of the same workload (per launch)
-        traffic = None
-        try:
-            if args.size == "8k" and args.kind == "photo" and headline:
-                tj = json.load(open(os.path.join(ROOT, "profiles", "traffic_8k_photo.json")))["kernels"]
-                # the kernels of the stage (K2 = two launches: the coder and k_huff_place; its time above covers both)
-                names = {"k1_fdct": ("k_fdct_rgb444",), "k2_huffman_encode": ("k_huff_encode", "k_huff_place"),
-                         "k3_huffman_decode": ("k_huff_decode",), "k4_idct": ("k_idct_rgb444",)}[worst]
-                hits = [v for k, v in tj.items() if k.startswith(names)]
-                if hits:
-                    traffic = int(sum(v["dram_bytes_read"] + v["dram_bytes_write"] for v in hits))
-        except Exception:
-            traffic = None
         roof = {k: alg[k] * npix / (stages[k] * 1e-3) / 1e9 for k in stages}
         path_gbs = (6.0 + 4 * coef_bpp + 2 * c_bpp) * npix / (ms_step * 1e-3) / 1e9
         line = {
@@ -637,7 +670,7 @@ def main():
                        "sharding": "one coder instance per GPU, independent frames, no data-path collective"},
             "stage_ms": {k: round(v, 4) for k, v in stages.items()},
             "roofline": {"bound": "hbm", "kernel": worst, "achieved": round(roof[worst], 1), "peak": peak, "unit": "GB/s",
-                         "frac": round(roof[worst] / peak, 4), "traffic": traffic, "peak_source": peak_kind,
+                         "frac": round(roof[worst] / peak, 4), "peak_source": peak_kind,
                          "all_stages_gbs": {k: round(v, 1) for k, v in roof.items()},
                          "path_achieved_gbs": round(path_gbs, 1), "path_frac": round(path_gbs / peak, 4)},
             "e2e": {"value": round(e2e_value, 1), "unit": "Mpix/s", "ms_per_step": round(e2e_ms, 3),
@@ -653,6 +686,7 @@ def main():
             # per step: K1, K2 (encode, offsets, compaction), K0 (count, scan, write), K3, K4 -- plus one 32-byte memset node
             "gpu_launches": 6 * args.steps,
             "clocks": clocks,
+            "device": device_line(local),
         }
         if not args.no_reference_gpu and world == 1:
             line["extras"] = {"reference_gpu": reference_gpu(args.kind, width, height, rst)}

@@ -95,6 +95,7 @@ def _load():
         "gpujpeg_decoder_get_stats": (ci, [vp, C.POINTER(DurationStats)]),
         "gpujpeg_decoder_get_image_info": (ci, [vp, cs, C.POINTER(ImageParameters), C.POINTER(Parameters), C.POINTER(ci)]),
         "gpujpegx_encoder_get_coefficients": (ci, [vp, vp, cs]),
+        "gpujpegx_encoder_get_stream": (C.c_longlong, [vp, vp, cs]),
         "gpujpegx_encoder_run_resident": (ci, [vp, vp, ci]),
         "gpujpegx_decoder_run_resident": (ci, [vp, vp, ci]),
         "gpujpegx_decoder_get_coefficients": (ci, [vp, vp, cs]),
@@ -244,6 +245,14 @@ class Encoder:
         addr = _ptr(d_raw)[0] if d_raw is not None else None
         if lib.gpujpegx_encoder_run_resident(self._h, addr, stage_mask) != 0:
             raise GpuJpegError("gpujpegx_encoder_run_resident failed")
+
+    def stream(self):
+        """the JPEG bytes the last K2 launch produced (after run_resident too), as gpujpeg_encoder_encode returns them"""
+        n = lib.gpujpegx_encoder_get_stream(self._h, None, 0)
+        out = np.empty(max(n, 0), np.uint8)
+        if n < 0 or lib.gpujpegx_encoder_get_stream(self._h, out.ctypes.data, out.size) != n:
+            raise GpuJpegError("gpujpegx_encoder_get_stream failed")
+        return out
 
     def coefficients(self, width, height, sampling=(1, 1), interleaved=0):
         """quantised coefficients of the last frame, natural order (parity tests): (3, blocks*64) int16 for 4:4:4,

@@ -1,6 +1,6 @@
-"""Builds gpujpeg_b200/lib/libgpujpeg.so.0 -- the drop-in C-ABI library -- for sm_100a.
+"""Builds gpujpeg_b200/lib/libgpujpeg.so.0 -- the drop-in C-ABI library -- for sm_90a (H100).
 
-Host files are C (gcc), kernels are CUDA (nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo),
+Host files are C (gcc), kernels are CUDA (nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo),
 the CUDA runtime is linked statically so the .so is self-contained next to torch's own runtime.
 nvcc cross-compiles without a GPU, so this runs in the build container; the built .so is
 git-ignored but travels to the GPU box with the repo snapshot.
@@ -19,7 +19,7 @@ LIB = os.path.join(LIBDIR, SONAME)
 
 C_SOURCES = ["gj_tables.c", "gj_codestream.c", "gj_common.c", "gj_imageio.c", "gj_exif.c", "gj_encoder.c", "gj_decoder.c", "gj_batch.c"]
 CU_SOURCES = ["gj_cuda_util.cu", "gj_dct.cu", "gj_huffman.cu", "gj_huffdec.cu", "gj_markers.cu", "gj_convert.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _nvcc():

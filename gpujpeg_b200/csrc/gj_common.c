@@ -92,8 +92,8 @@ int gpujpeg_init_device(int device_id, int flags)
         GJ_ERR("Can't get CUDA device properties!\n");
         return -1;
     }
-    if ( d.cc_major < 10 ) {
-        GJ_ERR("Device %d (%s, c.c. %d.%d) is not a Blackwell GPU: this build carries sm_100a code only.\n", device_id,
+    if ( d.cc_major != 9 || d.cc_minor != 0 ) {
+        GJ_ERR("Device %d (%s, c.c. %d.%d) is not a c.c. 9.0 Hopper GPU: this build carries sm_90a code only.\n", device_id,
                d.name, d.cc_major, d.cc_minor);
         return -1;
     }

@@ -1,5 +1,5 @@
 /*
- * gj_convert.cu -- generic pre-/post-processing pass (sm_100a): any supported pixel format in any of the colour spaces
+ * gj_convert.cu -- generic pre-/post-processing pass (sm_90a): any supported pixel format in any of the colour spaces
  * RGB / YCbCr BT.601 / YCbCr BT.601 full range / YCbCr BT.709 to and from the component planes of a YCbCr JPEG with any
  * supported sampling.
  *

@@ -1,5 +1,5 @@
 /*
- * gj_dct.cu -- the two transform kernels of the hot path (sm_100a).
+ * gj_dct.cu -- the two transform kernels of the hot path (sm_90a).
  *
  *   K1  k_fdct_rgb444 : RGB u8 interleaved -> int16 zig-zag coefficients
  *       = colour transform + component split + 8x8 forward DCT + quantisation in ONE pass over HBM
@@ -16,7 +16,7 @@
  * blocks (512 x 8 pixels), 192 threads.  In the transform phase thread t owns block (t % 64) of
  * component (t / 64) entirely in registers: both 1-D passes run without any transpose or shuffle,
  * which matters because the arithmetic has to follow the reference's rounding sequence exactly and
- * these kernels are instruction-issue bound, not bandwidth bound (ncu, profiles/r1_a).  In the colour
+ * these kernels are instruction-issue bound, not bandwidth bound.  In the colour
  * phase every thread handles 4 pixels = 12 interleaved bytes = three 32-bit words, read from / written
  * to global memory directly (a warp touches 384 contiguous bytes); the only shared-memory traffic is
  * the planar staging area between the two phases.  No conversion-pipe (XU) instruction is used for
@@ -836,10 +836,10 @@ static int launch_fdct_rgb444(const uint8_t* d_raw, int width, int height, int p
             return -1;
         __atomic_store_n(&attr_done[dev], 1, __ATOMIC_RELEASE);
     }
-    /* Two ways of getting the pixels on chip.  Measured on B200, 8K (profiles/r2_k1_bulk_vs_ldg.md): plain coalesced loads
-     * 133.2 us, copy-engine bulk copies into a persistent CTA 140.5 us -- the kernel is bound by instruction issue, not by
-     * the loads, and the bulk variant pays two CTA-wide barriers per strip at 3 instead of 4 CTAs per SM.  The plain-load
-     * kernel is the default; GPUJPEG_B200_K1=bulk selects the other one (rows must be 16-byte aligned). */
+    /* Two ways of getting the pixels on chip: plain coalesced loads, or copy-engine bulk copies into a persistent CTA
+     * (profiles/k1_times.py times both).  The kernel is bound by instruction issue, not by the loads, and the bulk variant
+     * pays two CTA-wide barriers per strip at 3 instead of 4 CTAs per SM.  The plain-load kernel is the default;
+     * GPUJPEG_B200_K1=bulk selects the other one (rows must be 16-byte aligned). */
     static int use_bulk = -1;
     if ( use_bulk < 0 ) {
         const char* e = getenv("GPUJPEG_B200_K1");
@@ -852,7 +852,7 @@ static int launch_fdct_rgb444(const uint8_t* d_raw, int width, int height, int p
             if ( cudaFuncSetAttribute(k_fdct_rgb444_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, K1T_SMEM) != cudaSuccess ) return -1;
             __atomic_store_n(&bulk_attr[dev], 1, __ATOMIC_RELEASE);
         }
-        int sms = 148;
+        int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         const int n_strips = (int)grid.x * (int)grid.y;
         const int ctas = n_strips < sms * 3 ? n_strips : sms * 3;   // 3 CTAs of 64.5 KB per SM

@@ -1,5 +1,5 @@
 /*
- * gj_decoder.c -- the public decoder API on top of the sm_100a stage launchers.  Host C.
+ * gj_decoder.c -- the public decoder API on top of the sm_90a stage launchers.  Host C.
  *
  * Contract of the reference orchestrator (src/gpujpeg_decoder.c:94-469): lazily (re)initialises
  * from the stream, one CUDA stream, blocks until the pixels are where the output descriptor says.
@@ -8,7 +8,7 @@
  *     host reader: marker segments only (headers, SOS); the file is uploaded ONCE, untouched, and the
  *                  restart markers are found by K0 on the device -- the reference walks the whole stream
  *                  with memchr and re-packs it segment by segment (src/gpujpeg_reader.c:1038-1155),
- *                  which alone costs 2.1 ms for an 8K frame on a B200 host (profiles/r1_b)
+ *                  which alone costs several times the GPU time of the whole decode at 8K
  *     H2D file bytes -> K0 marker list -> (tiny D2H, sync) -> host finishes the marker walk
  *       -> K3 Huffman decode (always on the GPU: no "fewer than 32 segments => CPU" fallback,
  *          src/gpujpeg_decoder.c:254-286)
@@ -525,20 +525,20 @@ static int resync_segments(struct gpujpeg_decoder* d, const struct gj_stream* st
     return rc;
 }
 
-/* Which Huffman decoder kernel (measured on B200, profiles/r2_k3_matrix.md): a frame with few segments cannot occupy the
- * GPU with one thread per segment -- there the self-synchronising walks buy parallelism INSIDE a segment (HD: 27 us
- * against 82, 4K: 41 against 90); with 40 000 segments and more the segments alone keep the machine busy and the redundant
- * walks pay off from photographic densities on (8K q75: 119 us against 174, q90: 268 against 332), not for very sparse
- * (q50: 97 either way) or random content (562 against 731).  Interleaved scans: a walk that starts inside the stream also
- * has to guess which component's block it is in, and a wrong guess does not heal by itself (other Huffman tables) --
- * exactness then spreads one lane per round; one thread per segment is faster at every size measured (8K 4:2:0: 150 us
- * against 258, 4K: 108 / 170, HD: 97 / 99). */
+/* Which Huffman decoder kernel (both timed by frame size and content with profiles/k3_matrix.py on an H100 SXM): a frame
+ * with few segments cannot occupy the GPU with one thread per segment -- there the self-synchronising walks buy
+ * parallelism INSIDE a segment (4K photo: 66 us against 102); with 30 000 segments and more the segments alone keep the
+ * machine busy and the redundant walks pay off only for dense segments, 8 to 20 bytes per block (8K q90: 330 us with 32
+ * lanes against 401), not at photographic q75 densities (8K: 205 against 212 with the best lane count), for very sparse
+ * or for random content.  Interleaved scans: a walk that starts inside the
+ * stream also has to guess which component's block it is in, and a wrong guess does not heal by itself (other Huffman
+ * tables) -- exactness then spreads one lane per round; one thread per segment is faster at every size. */
 static int wants_thread_per_segment(const struct gpujpeg_decoder* d, const struct gj_geometry* g, size_t ecs_bytes)
 {
     const size_t bytes_per_block_x10 = ecs_bytes * 10 / (g->coef_count / 64);
     const int many_segments = g->seg_count >= 30000;
     return d->thread_per_segment || g->lay.interleaved || g->seg_mcu * g->lay.bpm > 40 ||
-           (many_segments && (bytes_per_block_x10 < 20 || bytes_per_block_x10 > 200));
+           (many_segments && (bytes_per_block_x10 < 80 || bytes_per_block_x10 > 200));
 }
 
 /* Segment info [ref: src/gpujpeg_reader.c:1168-1215]: a stream can carry, in front of every scan, the position of every
@@ -924,7 +924,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     ha.d_list_cpos = d->d_list_cpos;
     ha.force_thread_per_segment = d->thread_per_segment;
     /* which kernel (wants_thread_per_segment), and for the self-synchronising one how many lanes share a restart segment
-     * (profiles/r2_k3_matrix.md) */
+     * (profiles/k3_matrix.py) */
     size_t ecs_bytes = 0;
     for ( int k = 0; k < g->scan_count; k++ )
         ecs_bytes += st.scan[k].end - st.scan[k].begin;
@@ -938,7 +938,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         const size_t avg = (st.scan[k].end - st.scan[k].begin) / (size_t)segs;
         ha.scan_lanes[k] = (uint8_t)(g->seg_count <= 8000 ? 16
                                      : !many_segments     ? (bytes_per_block_x10 > 100 ? 16 : 8)
-                                     : bytes_per_block_x10 > 80 ? 8 : avg >= 192 ? 16 : 8);
+                                     : 32);
         if ( d->force_lanes[k] ) {   /* (never with by_table: split_by_segment_info declines then) */
             ha.scan_lanes[k] = (uint8_t)d->force_lanes[k];
             ha.force_thread_per_segment = d->thread_per_segment;

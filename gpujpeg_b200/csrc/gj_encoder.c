@@ -1,5 +1,5 @@
 /*
- * gj_encoder.c -- the public encoder API on top of the sm_100a stage launchers.  Host C.
+ * gj_encoder.c -- the public encoder API on top of the sm_90a stage launchers.  Host C.
  *
  * Mirrors the reference orchestrator's contract (src/gpujpeg_encoder.c:351-646): same parameter
  * handling (comp_count 0 => from pixel format, RESTART_AUTO heuristic), same re-initialisation
@@ -1065,6 +1065,22 @@ GPUJPEG_API int gpujpegx_encoder_run_resident(struct gpujpeg_encoder* e, const u
     if ( (stage_mask & 1) && launch_k1(e, d_raw) ) return -1;
     if ( (stage_mask & 2) && launch_k2(e) ) return -1;
     return 0;
+}
+
+/* ---- extension used by bench.py: the JPEG stream the last K2 launch produced (resident re-runs included) ---- */
+GPUJPEG_API long long gpujpegx_encoder_get_stream(struct gpujpeg_encoder* e, uint8_t* out, size_t capacity)
+{
+    if ( !e || !e->initialised || e->with_segment_info || !e->d_info_cur ) return -1;
+    if ( gj_cuda_memcpy_d2h_async(e->h_info, e->d_info_cur, 32, e->stream) || gj_cuda_stream_sync(e->stream) ) return -1;
+    const size_t total = (size_t)e->h_info[0];
+    if ( e->h_info[1] || total < e->header_size + 2 || total > e->d_stream_size ) return -1;
+    if ( !out ) return (long long)total;
+    if ( total > capacity ) return -1;
+    if ( gj_cuda_memcpy_d2h_async(out + e->header_size, e->d_stream + e->header_size, total - e->header_size, e->stream) ||
+         gj_cuda_stream_sync(e->stream) )
+        return -1;
+    memcpy(out, e->header, e->header_size);
+    return (long long)total;
 }
 
 /* ---- extension used by the parity tests: quantised coefficients of the last frame, natural order ---- */

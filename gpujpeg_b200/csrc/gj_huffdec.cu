@@ -1,5 +1,5 @@
 /*
- * gj_huffdec.cu -- K3: self-synchronising, restart-interval-parallel Huffman decoder (sm_100a).
+ * gj_huffdec.cu -- K3: self-synchronising, restart-interval-parallel Huffman decoder (sm_90a).
  *
  * The reference decodes one restart segment per THREAD (src/gpujpeg_huffman_gpu_decoder.cu:390-537): 43 200 threads
  * for an 8K frame, each walking a few hundred symbols one after the other.  The first decoder of this repository
@@ -928,7 +928,7 @@ extern "C" int gj_launch_huffman_decode_sync(const struct gj_huff_dec_args* a, g
             if ( sb > stage_bytes ) stage_bytes = sb;
         }
     }
-    int sms = 148;
+    int sms = 132;
     int dev = 0;
     if ( cudaGetDevice(&dev) != cudaSuccess ) return -1;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);

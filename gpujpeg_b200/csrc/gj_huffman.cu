@@ -1,5 +1,5 @@
 /*
- * gj_huffman.cu -- restart-interval-parallel Huffman encoder and decoder (sm_100a).
+ * gj_huffman.cu -- restart-interval-parallel Huffman encoder and decoder (sm_90a).
  *
  * ENCODER (replaces the reference's three kernels src/gpujpeg_huffman_gpu_encoder.cu:299-404,
  * 416-502, 562-615 and the host re-ordering loop src/gpujpeg_encoder.c:567-626):
@@ -775,10 +775,7 @@ constexpr int HD_THREADS = 128;
 #ifndef GJ_HD_SPW
 #define GJ_HD_SPW 16
 #endif
-/* measured on B200, photo-like / random content, owners per warp 32 | 16 | 8 | 4:
- *   8K  (43 200 segments)  207/538 | 190/526 | 189/878 | 255/1318 us   -> 16
- *   4K  (16 200 segments)     -    | 111/291 | 103/289 |  95/365  us   -> 8
- *   HD  ( 4 050 segments)     -    | 109/277 |  95/253 |  83/239  us   -> 4 */
+/* segment owners per warp: fewer for frames with fewer segments (profiles/k3_matrix.py times the choices) */
 constexpr int HD_SEGMENTS_PER_WARP = GJ_HD_SPW;
 
 struct DecTabs {

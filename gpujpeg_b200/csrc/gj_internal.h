@@ -1,8 +1,8 @@
 /*
- * gj_internal.h -- internal structures of the B200-native libgpujpeg replacement.
+ * gj_internal.h -- internal structures of the H100-native libgpujpeg replacement.
  *
  * Host code is plain C (north_star: "host code stays C calling into a thin C-ABI layer of
- * hand-written sm_100a CUDA kernels").  The stage launchers at the bottom are that thin layer:
+ * hand-written sm_90a CUDA kernels").  The stage launchers at the bottom are that thin layer:
  * extern "C", plain pointers and sizes, implemented in the .cu files.
  *
  * Data layout in HBM (see DESIGN.md section 3):
@@ -67,7 +67,7 @@ void gj_enc_lut_build(const struct gj_huff_spec* dc, const struct gj_huff_spec* 
  *   maxcode[l]  = exclusive upper bound of all codes of length <= l, left-justified to 16 bits
  *   valoff[l]   = valptr[l] - mincode[l]
  *   vals[]      = HUFFVAL
- * (a two-level table and a cp.async staging ring were measured as well, profiles/r1_e: both lengthen the
+ * (a two-level table and a cp.async staging ring were measured as well: both lengthen the
  * per-warp instruction stream, which is what bounds the decoder, and lost against this variant) */
 #define GJ_DEC_LOOK_BITS 9
 struct gj_dec_lut {
@@ -468,7 +468,7 @@ void gj_timer_start(struct gj_timer* t, gj_stream_t s);
 void gj_timer_stop(struct gj_timer* t, gj_stream_t s);
 double gj_timer_ms(struct gj_timer* t);
 int gj_cuda_device_count(void);
-int gj_cuda_sm_count(void);   /* multiprocessors of the current device (148 on a B200); 1 on failure */
+int gj_cuda_sm_count(void);   /* multiprocessors of the current device (132 on an H100 SXM); 1 on failure */
 int gj_cuda_device_props(int dev, struct gpujpeg_device_info* info);
 int gj_cuda_set_device(int dev);
 int gj_cuda_get_device(void);

@@ -7,9 +7,9 @@
  * kernel -- until the previous grid has completed and its writes are visible.  Because every kernel of the chain waits
  * before it touches memory, the order of all memory operations is the plain stream order.  A kernel launched this way behind
  * something that is not a kernel (memset, copy) is serialised as usual; GPUJPEG_B200_PDL=0 turns the attribute off.
- * Measured on B200, 8K frame, six kernels per step: 0.471 -> 0.457 ms.  Letting the dependents become resident earlier
- * (`griddepcontrol.launch_dependents` at the top of every kernel, table copies in front of the wait) made every stage
- * faster when timed alone and the chain slower (0.464 ms): waiting CTAs share the SMs with the grid that still works.
+ * Letting the dependents become resident earlier (`griddepcontrol.launch_dependents` at the top of every kernel, table
+ * copies in front of the wait) made every stage faster when timed alone and the chain slower: waiting CTAs share the SMs
+ * with the grid that still works.
  */
 #ifndef GJ_LAUNCH_CUH
 #define GJ_LAUNCH_CUH

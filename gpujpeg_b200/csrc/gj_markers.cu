@@ -6,8 +6,8 @@
  *
  * The reference splits scans into restart segments on the host with a memchr(0xFF) walk over the whole
  * stream and copies every segment into a second buffer (src/gpujpeg_reader.c:1038-1155); its FAQ quotes
- * 543 ms for that step on one sample.  On a B200 host the same walk costs 2.1 ms for an 8K frame --
- * six times the GPU time of the entire decode.  Here the file is uploaded once, untouched, and ONE launch does the
+ * 543 ms for that step on one sample; for an 8K frame the same walk costs several times the GPU time of the
+ * entire decode.  Here the file is uploaded once, untouched, and ONE launch does the
  * reader's per-byte work in device memory (k_marker_scan_write): every CTA classifies a 4 KB tile (16 bytes per
  * thread), counts its markers and the bytes that stay in the clean stream, publishes both, adds up what the tiles in
  * front of it have published (no chain: every tile sums its predecessors' counts itself, ~3 loads per thread on average

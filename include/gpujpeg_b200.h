@@ -1,5 +1,5 @@
 /*
- * gpujpeg_b200.h -- the C ABI of the B200-native JPEG hot path.
+ * gpujpeg_b200.h -- the C ABI of the H100-native JPEG hot path.
  *
  * This single header declares, in one place, every type and entry point that a
  * caller of libgpujpeg binds against.  It is written from scratch (no text

@@ -1,5 +1,5 @@
 /*
- * gpujpegx.h -- extension entry points of the B200-native libgpujpeg (additive: nothing here exists in the reference;
+ * gpujpegx.h -- extension entry points of the H100-native libgpujpeg (additive: nothing here exists in the reference;
  * every name carries the prefix gpujpegx_).  The reference API itself is in libgpujpeg/gpujpeg.h.
  *
  *   * resident re-runs and coefficient read-back: used by bench.py and the parity tests
@@ -26,6 +26,10 @@ GPUJPEG_API int gpujpegx_encoder_run_resident(struct gpujpeg_encoder* encoder, c
 /* stage_mask: bit 2 = K0 (marker list + clean stream from the JPEG bytes on the device), bit 0 = K3 (Huffman decode),
  * bit 1 = K4 (dequantisation + IDCT + colour); d_out == NULL writes into the decoder's own buffer */
 GPUJPEG_API int gpujpegx_decoder_run_resident(struct gpujpeg_decoder* decoder, uint8_t* d_out, int stage_mask);
+/* the JPEG stream of the last frame as the last K2 launch left it (resident re-runs included), the same bytes
+ * gpujpeg_encoder_encode returns: its size, copied into `out` when `out` is not NULL and holds it; -1 on error or when
+ * the encoder writes segment-info tables (those are completed on the host) */
+GPUJPEG_API long long gpujpegx_encoder_get_stream(struct gpujpeg_encoder* encoder, uint8_t* out, size_t capacity);
 /* quantised coefficients of the last frame, natural order, block-major (parity tests).  The decoder variant returns 1
  * when the values are already multiplied by the quantiser (integer IDCT flavour), 0 otherwise, -1 on error */
 GPUJPEG_API int gpujpegx_encoder_get_coefficients(struct gpujpeg_encoder* encoder, int16_t* out, size_t count);

@@ -1,7 +1,7 @@
-"""Turns an ncu --set full report into the two committed summaries:
-    python profiles/export_summary.py gpurun_out/prof_r1_k.ncu-rep r1_k
- -> profiles/<tag>_ncu_full_summary.csv  (one column per kernel, the metrics DESIGN.md / README.md quote)
- -> profiles/<tag>_traffic.json and profiles/traffic_8k_photo.json (DRAM bytes per launch; bench.py reads the latter)"""
+"""Turns an ncu --set full report into two summaries (profiles/out/ is kept out of git):
+    python profiles/export_summary.py <report>.ncu-rep <tag>
+ -> profiles/out/<tag>_ncu_full_summary.csv  (one column per kernel)
+ -> profiles/out/<tag>_traffic.json (DRAM bytes per launch)"""
 import csv
 import json
 import os
@@ -37,7 +37,9 @@ names = []
 for r in data:
     n = re.sub(r"\(.*", "", r[idx["Kernel Name"]]).replace("void ", "").replace("<unnamed>::", "").strip()
     names.append(n)
-with open(os.path.join(HERE, tag + "_ncu_full_summary.csv"), "w", newline="") as f:
+OUT = os.path.join(HERE, "out")
+os.makedirs(OUT, exist_ok=True)
+with open(os.path.join(OUT, tag + "_ncu_full_summary.csv"), "w", newline="") as f:
     w = csv.writer(f)
     w.writerow(["metric", "unit"] + names)
     for k in KEEP:
@@ -53,6 +55,5 @@ for n, r in zip(names, data):
     dur, du = float(r[idx["gpu__time_duration.sum"]]), units[idx["gpu__time_duration.sum"]]
     traffic["kernels"][n] = {"dram_bytes_read": val("dram__bytes_read.sum"), "dram_bytes_write": val("dram__bytes_write.sum"),
                              "duration_us_under_ncu": dur * {"us": 1.0, "ns": 1e-3, "ms": 1e3}.get(du, 1.0)}
-for out in (tag + "_traffic.json", "traffic_8k_photo.json"):
-    json.dump(traffic, open(os.path.join(HERE, out), "w"), indent=1)
+json.dump(traffic, open(os.path.join(OUT, tag + "_traffic.json"), "w"), indent=1)
 print(json.dumps(traffic["kernels"], indent=1))

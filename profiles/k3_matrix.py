@@ -1,4 +1,4 @@
-"""K3 alone (Huffman decode) by frame size, content, quality, kernel and lanes per segment -> gpurun_out/k3_matrix.json
+"""K3 alone (Huffman decode) by frame size, content, quality, kernel and lanes per segment -> profiles/out/k3_matrix.json
     python profiles/k3_matrix.py [quick]
 CUDA events over 20 launches after 3 warm-up launches; every configuration is first decoded through the public call and
 compared with the default configuration's output (identical pixels)."""
@@ -49,5 +49,5 @@ for size, kind, q in CASES:
         dec.close()
     rows.append(row)
     print(json.dumps(row), flush=True)
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-json.dump(rows, open(os.path.join(ROOT, "gpurun_out", "k3_matrix.json"), "w"), indent=1)
+os.makedirs(os.path.join(ROOT, "profiles", "out"), exist_ok=True)
+json.dump(rows, open(os.path.join(ROOT, "profiles", "out", "k3_matrix.json"), "w"), indent=1)

@@ -2,7 +2,7 @@
 import csv, os, re, subprocess, sys, tempfile
 rep, kern, stem = sys.argv[1], sys.argv[2], sys.argv[3]
 ranges = [tuple(int(x) for x in r.split("-")) for r in sys.argv[4:]]
-ROOT = "/root/repo"
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "gpujpeg_b200", "lib", "libgpujpeg.so.0")
 tmp = tempfile.mkdtemp()
 subprocess.run(["cuobjdump", "-xelf", "all", lib], cwd=tmp, capture_output=True)

@@ -1,5 +1,6 @@
 """ctypes bindings for the CPU oracle (oracle/liboracle.so) and, when present, the reference's own
-CPU code compiled in place (oracle/_ref/libgpujpeg_refcpu.so).  Test infrastructure only."""
+CPU code compiled in place (oracle/_ref/libgpujpeg_refcpu.so, used to record tests/golden/refcpu_answers.npz).
+Test infrastructure only."""
 import ctypes as C
 import os
 import subprocess
@@ -319,6 +320,12 @@ if os.path.exists(_REF_SO):
                                             C.c_size_t]
     ref.ref_encode_from_coef_cs.restype = C.c_size_t
     ref.ref_idct_block.argtypes = [_i16p, np.ctypeslib.ndpointer(np.uint16)]
+    ref.ref_encode_from_coef_rgb_n.argtypes = [_i16p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _u8p, C.c_size_t]
+    ref.ref_encode_from_coef_rgb_n.restype = C.c_size_t
+    ref.ref_set_header_type.argtypes = [C.c_int]
+    ref.ref_set_orientation.argtypes = [C.c_int, C.c_int, C.c_int]
+    ref.ref_add_exif_tag.argtypes = [C.c_char_p]
+    ref.ref_exif_parse.argtypes = [_u8p, C.c_size_t]
 
 
 def remap_code(val):

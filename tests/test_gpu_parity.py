@@ -1,6 +1,6 @@
 """GPU parity tests proper: the CUDA path, called through the C ABI (gpujpeg_encoder_encode /
 gpujpeg_decoder_decode), against the CPU oracle on the same seeded inputs -- bit-exact.
-Run on the B200 box:  python -m pytest tests -m gpu"""
+Run on an H100:  python -m pytest tests -m gpu"""
 import glob
 import os
 

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import _oracle as o
+from _refcpu import answer
 from _shims import io
 
 U8, P012, P0P1P2_444, P1020, P0P1P2_422, P0P1P2_420, P0123 = range(7)
@@ -115,16 +116,32 @@ def test_netpbm_save_load(tmp_path, ext, fmt, cs, depth, head):
     rc, p = _props(path)
     assert rc == 0 and (p.width, p.height, p.pixel_format) == (w, h, fmt)
     assert p.color_space == (BT601_256 if depth == 1 else RGB)
-    if o.ref is not None:
-        ref_path = tmp_path / ("ref." + ext)
-        assert o.ref.pam_write(str(ref_path).encode(), w, w, h, depth, 255, data.ctypes.data, ext != "pam")
-        assert ref_path.read_bytes() == raw                  # byte-identical files
+    ref_path = tmp_path / ("ref." + ext)
+
+    def ref_save():
+        ok = o.ref.pam_write(str(ref_path).encode(), w, w, h, depth, 255, data.ctypes.data, ext != "pam")
+        return ok, np.frombuffer(ref_path.read_bytes(), np.uint8)
+    ok, ref_file = answer("pam_write", (ext, w, h, depth, data), ref_save, (None, np.frombuffer(raw, np.uint8)))
+    assert ok and ref_file.tobytes() == raw                  # byte-identical files
+    ok, meta, got = _ref_pam_read(path, data.size, expect=data)
+    assert ok and meta == (w, h, depth, 255)
+    assert np.array_equal(got, data)
+
+
+def _ref_pam_read(path, size=0, expect=None):
+    """pam_read of the reference on the file `path`: (ok, (width, height, channels, maxval), the first `size` samples)"""
+    def compute():
         m, ptr = PamMeta(), C.c_void_p()
-        assert o.ref.pam_read(str(path).encode(), C.byref(m), C.byref(ptr), _malloc)
-        assert (m.width, m.height, m.ch_count, m.maxval) == (w, h, depth, 255)
-        got = np.ctypeslib.as_array(C.cast(ptr, C.POINTER(C.c_uint8)), (data.size,)).copy()
-        _libc.free(ptr)
-        assert np.array_equal(got, data)
+        ok = o.ref.pam_read(str(path).encode(), C.byref(m), C.byref(ptr) if size else None, _malloc if size else _ALLOC(0))
+        got = np.zeros(0, np.uint8)
+        if ok and size:
+            got = np.ctypeslib.as_array(C.cast(ptr, C.POINTER(C.c_uint8)), (size,)).copy()
+        if ptr.value:
+            _libc.free(ptr)
+        return ok, np.array([m.width, m.height, m.ch_count, m.maxval]), got
+    ok, meta, got = answer("pam_read", (os.path.basename(path), np.frombuffer(path.read_bytes(), np.uint8), size), compute,
+                           (None, None, expect))
+    return bool(ok), tuple(int(v) for v in np.atleast_1d(meta)), got
 
 
 def test_netpbm_headers_with_comments(tmp_path):
@@ -141,11 +158,9 @@ def test_netpbm_headers_with_comments(tmp_path):
     assert rc == 0 and (pr.width, pr.height, pr.pixel_format) == (5, 4, P0123)
     rc, back = _load(q)
     assert rc == 0 and back.size == 80
-    if o.ref is not None:
-        for f, n in ((p, 3), (q, 4)):
-            m = PamMeta()
-            assert o.ref.pam_read(str(f).encode(), C.byref(m), None, _ALLOC(0))
-            assert (m.width, m.height, m.ch_count, m.maxval) == (5, 4, n, 255)
+    for f, n in ((p, 3), (q, 4)):
+        ok, meta, _ = _ref_pam_read(f)
+        assert ok and meta == (5, 4, n, 255)
 
 
 @pytest.mark.parametrize("content,why", [
@@ -168,9 +183,8 @@ def test_netpbm_refused(tmp_path, content, why):
     if why != "samples missing":
         rc, _ = _props(p)
         assert rc < 0, why
-    if o.ref is not None and why not in ("16-bit samples", "bitmap", "sizes whose product wraps", "wider than a JPEG can be"):   # (pam.c reads those; the delegates then refuse everything but 255 levels)
-        m, ptr = PamMeta(), C.c_void_p()
-        assert not o.ref.pam_read(str(p).encode(), C.byref(m), C.byref(ptr), _malloc), why
+    if why not in ("16-bit samples", "bitmap", "sizes whose product wraps", "wider than a JPEG can be"):   # (pam.c reads those; the delegates then refuse everything but 255 levels)
+        assert not _ref_pam_read(p, 1)[0], why
 
 
 def test_netpbm_save_rules(tmp_path):
@@ -201,15 +215,30 @@ def test_y4m_save_load(tmp_path, fmt, cs, chroma, rng, ss, w, h):
     rc, p = _props(path)
     assert rc == 0 and (p.width, p.height, p.pixel_format) == (w, h, fmt)
     assert p.color_space == (BT601 if rng == "LIMITED" else BT601_256)
-    if o.ref is not None:
-        ref_path = tmp_path / "ref.y4m"
+    ref_path = tmp_path / "ref.y4m"
+
+    def ref_save():
         m = Y4mMeta(w, h, 8, ss, rng == "LIMITED")
-        assert o.ref.y4m_write(str(ref_path).encode(), C.byref(m), data.ctypes.data)
-        assert ref_path.read_bytes() == raw
-        m2, ptr = Y4mMeta(), C.c_void_p()
-        assert o.ref.y4m_read(str(path).encode(), C.byref(m2), C.byref(ptr), _malloc) == n
-        assert (m2.width, m2.height, m2.bitdepth, m2.subsampling, m2.limited) == (w, h, 8, ss, rng == "LIMITED")
-        _libc.free(ptr)
+        ok = o.ref.y4m_write(str(ref_path).encode(), C.byref(m), data.ctypes.data)
+        return ok, np.frombuffer(ref_path.read_bytes(), np.uint8)
+    ok, ref_file = answer("y4m_write", (w, h, ss, rng, data), ref_save, (None, np.frombuffer(raw, np.uint8)))
+    assert ok and ref_file.tobytes() == raw
+    got, meta = _ref_y4m_read(path, True)
+    assert got == n
+    assert meta == (w, h, 8, ss, rng == "LIMITED")
+
+
+def _ref_y4m_read(path, alloc):
+    """y4m_read of the reference on the file `path`: (its return value, (width, height, bit depth, subsampling, limited))"""
+    def compute():
+        m, ptr = Y4mMeta(), C.c_void_p()
+        got = o.ref.y4m_read(str(path).encode(), C.byref(m), C.byref(ptr) if alloc else None, _malloc if alloc else _ALLOC(0))
+        if ptr.value:
+            _libc.free(ptr)
+        return got, np.array([m.width, m.height, m.bitdepth, m.subsampling, int(m.limited)])
+    got, meta = answer("y4m_read", (np.frombuffer(path.read_bytes(), np.uint8), alloc), compute)
+    meta = [int(v) for v in np.atleast_1d(meta)]
+    return int(got), tuple(meta[:4]) + (bool(meta[4]),)
 
 
 def test_y4m_foreign_headers(tmp_path):
@@ -228,9 +257,8 @@ def test_y4m_foreign_headers(tmp_path):
         q = tmp_path / "bad.y4m"
         q.write_bytes(head + bytes(200))
         assert _props(q)[0] < 0, why
-        if o.ref is not None and why in ("no chroma tag: the reference does not assume 4:2:0", "FRAME with parameters", "magic"):
-            m = Y4mMeta()
-            assert o.ref.y4m_read(str(q).encode(), C.byref(m), None, _ALLOC(0)) == 0, why
+        if why in ("no chroma tag: the reference does not assume 4:2:0", "FRAME with parameters", "magic"):
+            assert _ref_y4m_read(q, False)[0] == 0, why
     assert _save(tmp_path / "x.y4m", _rand(w * h * 3), w, h, P012, BT601_256)[0] != 0     # packed format
     assert _save(tmp_path / "y.y4m", _rand(w * h * 3), w, h, P0P1P2_444, RGB)[0] != 0     # RGB
 

@@ -1,20 +1,16 @@
-"""Differential tests: oracle restatement vs the reference's own CPU sources compiled in place
-(oracle/_ref/libgpujpeg_refcpu.so).  Skipped when that library has not been built (it needs
-/root/reference at build time; the prebuilt .so travels to the GPU box).  CPU only."""
+"""Differential tests: oracle restatement vs the reference's own CPU sources (their answers stored in
+tests/golden/refcpu_answers.npz, see tests/_refcpu.py).  CPU only."""
 import numpy as np
 import pytest
 
 import _oracle as o
-from _refcpu import ref_decode_coef, ref_encode_coef, ref_idct_planes
-
-pytestmark = pytest.mark.skipif(o.ref is None, reason="oracle/_ref/libgpujpeg_refcpu.so not built")
+from _refcpu import answer, ref_decode_coef, ref_encode_coef, ref_idct_blocks, ref_idct_planes, ref_quant_tables, ref_write
 
 
 @pytest.mark.parametrize("q", [1, 10, 25, 50, 75, 90, 95, 100])
 def test_quant_tables(q):
     raw, fwd, inv = o.quant_tables(q)
-    r2, f2, i2 = np.zeros_like(raw), np.zeros_like(fwd), np.zeros_like(inv)
-    assert o.ref.ref_quant_tables(q, r2, f2, i2) == 0
+    r2, f2, i2 = ref_quant_tables(q)
     assert np.array_equal(raw, r2) and np.array_equal(inv, i2)
     assert np.array_equal(fwd.view(np.uint32), f2.view(np.uint32)), "forward float table must be bit-identical"
 
@@ -23,8 +19,11 @@ def test_quant_tables(q):
 def test_huffman_tables(cls, kind):
     code, size = np.zeros(256, np.uint16), np.zeros(256, np.uint8)
     o.lib.orc_huff_encoder_table(cls, kind, code, size)
-    c2, s2 = np.zeros(256, np.uint32), np.zeros(256, np.uint8)
-    o.ref.ref_huff_encoder_table(cls, kind, c2, s2)
+    def compute():
+        c2, s2 = np.zeros(256, np.uint32), np.zeros(256, np.uint8)
+        o.ref.ref_huff_encoder_table(cls, kind, c2, s2)
+        return c2, s2
+    c2, s2 = answer("huff_encoder_table", (cls, kind), compute)
     assert np.array_equal(code.astype(np.uint32), c2) and np.array_equal(size, s2)
 
 
@@ -38,9 +37,9 @@ CASES = [("random", 1920, 1080, 75, 24, 0), ("photo", 1920, 1080, 75, 24, 0), ("
 def test_encode_bytes_and_decode_coefficients(kind, w, h, q, rst, il):
     img = o.gen_image(kind, w, h)
     jpeg, coef = o.encode(img, q, rst, il, want_coef=True)
-    ref_jpeg = ref_encode_coef(coef, w, h, q, rst, il)
+    ref_jpeg = ref_encode_coef(coef, w, h, q, rst, il, expect=jpeg)
     assert np.array_equal(jpeg, ref_jpeg), "oracle bytes != reference header writer + CPU Huffman encoder"
-    ref_coef = ref_decode_coef(jpeg, w, h, rst, il)
+    ref_coef = ref_decode_coef(jpeg, w, h, rst, il, expect=coef)
     assert np.array_equal(ref_coef, coef), "reference CPU Huffman decoder must recover the encoder's coefficients"
     _, coef_dec = o.decode(jpeg, want_coef=True)
     assert np.array_equal(coef_dec, coef)
@@ -58,9 +57,9 @@ def test_subsampled_encode_bytes_and_decode_coefficients(kind, w, h, q, rst, sam
     oracle against the reference's header writer + CPU Huffman coder [ref: src/gpujpeg_huffman_cpu_encoder.c:234-290]"""
     img = o.gen_image(kind, w, h)
     jpeg, coef = o.encode(img, q, rst, il, want_coef=True, sampling=sampling)
-    ref_jpeg = ref_encode_coef(coef, w, h, q, rst, il, sampling=sampling)
+    ref_jpeg = ref_encode_coef(coef, w, h, q, rst, il, sampling=sampling, expect=jpeg)
     assert np.array_equal(jpeg, ref_jpeg), "oracle bytes != reference header writer + CPU Huffman encoder"
-    ref_coef = ref_decode_coef(jpeg, w, h, rst, il, sampling=sampling)
+    ref_coef = ref_decode_coef(jpeg, w, h, rst, il, sampling=sampling, expect=coef)
     assert np.array_equal(ref_coef, coef), "reference CPU Huffman decoder must recover the encoder's coefficients"
     out, coef_dec = o.decode(jpeg, want_coef=True)
     assert np.array_equal(coef_dec, coef) and out.shape == (h, w, 3)
@@ -76,10 +75,8 @@ def test_rgb_internal_stream_bytes(il, sampling):
     jpeg = o.encode_any(img, w, h, o.FMT_444_P012, o.CS_RGB, q, rst, il, sampling, internal=o.CS_RGB)
     assert jpeg[2:4].tobytes() == b"\xff\xee" and b"Adobe" in jpeg[:20].tobytes()
     _, coef = o.decode(jpeg, want_coef=True)          # pixels are meaningless here (RGB samples), coefficients are not
-    out = np.empty(4096 + coef.size * 8, np.uint8)
-    n = o.ref.ref_encode_from_coef_rgb(np.ascontiguousarray(coef).reshape(-1), w, h, q, rst, il, sampling[0], sampling[1], out,
-                                       out.size)
-    assert n > 0 and np.array_equal(out[:n], jpeg)
+    ref_jpeg, _ = ref_write(coef, w, h, q, rst, il, sampling, internal=o.CS_RGB, expect=jpeg)
+    assert np.array_equal(ref_jpeg, jpeg)
     back = o.decode_any(jpeg, o.FMT_444_P012, o.CS_RGB).reshape(h, w, 3).astype(int)
     assert np.abs(back - img).mean() < 12
 
@@ -94,10 +91,8 @@ def test_spiff_stream_bytes(internal, il, sampling):
     jpeg = o.encode_any(img, w, h, o.FMT_444_P012, o.CS_RGB, q, rst, il, sampling, internal=internal)
     assert jpeg[2:4].tobytes() == b"\xff\xe8" and jpeg[6:12].tobytes() == b"SPIFF\x00"
     _, coef = o.decode(jpeg, want_coef=True)          # coefficients only; the pixels of o.decode assume YCbCr JPEG
-    out = np.empty(4096 + coef.size * 8, np.uint8)
-    n = o.ref.ref_encode_from_coef_cs(np.ascontiguousarray(coef).reshape(-1), w, h, q, rst, il, sampling[0], sampling[1],
-                                      internal, out, out.size)
-    assert n > 0 and np.array_equal(out[:n], jpeg)
+    ref_jpeg, _ = ref_write(coef, w, h, q, rst, il, sampling, internal=internal, expect=jpeg)
+    assert np.array_equal(ref_jpeg, jpeg)
     back = o.decode_any(jpeg, o.FMT_444_P012, o.CS_RGB).reshape(h, w, 3).astype(int)
     assert np.abs(back - img).mean() < 12
 
@@ -119,12 +114,13 @@ def test_integer_idct_matches_gpujpeg_idct_cpu(kind, q):
     w, h = 256, 128
     img = o.gen_image(kind, w, h)
     _, coef = o.encode(img, q, 8, want_coef=True)
-    planes = ref_idct_planes(coef, w, h, q)
     _, _, inv = o.quant_tables(q)
+    mine = np.zeros((3, h, w), np.uint8)
     for c in range(3):
-        plane = np.zeros(w * h, np.uint8)
-        o.lib.orc_idct_plane(np.ascontiguousarray(coef[c]), w, h, inv[0 if c == 0 else 1], o.IDCT_INT, plane)
-        assert np.array_equal(plane.reshape(h, w), planes[c])
+        o.lib.orc_idct_plane(np.ascontiguousarray(coef[c]), w, h, inv[0 if c == 0 else 1], o.IDCT_INT, mine[c])
+    planes = ref_idct_planes(coef, w, h, q, expect=mine)
+    for c in range(3):
+        assert np.array_equal(mine[c], planes[c])
 
 
 def test_idct_saturating_blocks():
@@ -132,6 +128,7 @@ def test_idct_saturating_blocks():
     1024-entry clip table (outside it the reference reads out of bounds, src/gpujpeg_dct_cpu.c:42-43)."""
     rng = np.random.default_rng(7)
     _, _, inv = o.quant_tables(50)
+    blocks = []
     for _ in range(3000):
         blk = np.zeros(64, np.int16)
         idx = rng.choice(64, 6, replace=False)
@@ -139,10 +136,12 @@ def test_idct_saturating_blocks():
         blk[0] = rng.integers(-24, 25)
         if np.abs(blk.astype(np.int64) * inv[0]).sum() > 1900:
             continue
-        a, b = blk.copy(), blk.copy()
+        blocks.append(blk)
+    blocks = np.array(blocks)
+    mine = blocks.copy()
+    for a in mine:
         o.lib.orc_idct_int_block(a, inv[0])
-        o.ref.ref_idct_block(b, inv[0])
-        assert np.array_equal(a, b)
+    assert np.array_equal(mine, ref_idct_blocks(blocks, inv[0], expect=mine))
 
 
 @pytest.mark.parametrize("hdr", [1, 2, 4])           # GPUJPEG_HEADER_JFIF, _SPIFF, _ADOBE
@@ -155,21 +154,7 @@ def test_forced_header_flavours_equal_the_reference_writer(hdr, internal):
     from _shims import hs
     w, h, q, rst = 64, 48, 75, 4
     coef = np.zeros((3, 64 * 48), np.int16)
-    o.ref.ref_set_header_type.argtypes = [__import__("ctypes").c_int]
-    o.ref.ref_set_header_type(hdr)
-    try:
-        if internal == 1:
-            out = np.empty(1 << 16, np.uint8)
-            n = o.ref.ref_encode_from_coef_rgb(coef.reshape(-1), w, h, q, rst, 0, 1, 1, out, out.size)
-        elif internal in (2, 4):
-            out = np.empty(1 << 16, np.uint8)
-            n = o.ref.ref_encode_from_coef_cs(coef.reshape(-1), w, h, q, rst, 0, 1, 1, internal, out, out.size)
-        else:
-            out = np.empty(1 << 16, np.uint8)
-            n = o.ref.ref_encode_from_coef_ss(coef.reshape(-1), w, h, 3, q, rst, 0, 1, 1, out, out.size)
-    finally:
-        o.ref.ref_set_header_type(0)
-    ref = bytes(out[:n])
+    ref = bytes(ref_write(coef, w, h, q, rst, 0, (1, 1), 3, internal=internal, header_type=hdr)[0])
     sos = ref.index(b"\xff\xda")
     got = np.zeros(4096, np.uint8)
     hs.shim_set_header_type(hdr)

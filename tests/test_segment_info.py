@@ -1,6 +1,6 @@
 """struct gpujpeg_parameters.segment_info: APP13 headers in front of every SOS with the byte position of every restart segment
 inside the scan [ref: src/gpujpeg_writer.c:522-599, src/gpujpeg_encoder.c:575-621].  The oracle's restatement is pinned
-against the reference GPU library on the B200 (tests/test_ref_gpu.py::test_reference_gpu_segment_info); here: the structure
+against the reference GPU library (tests/test_ref_gpu.py::test_reference_gpu_segment_info); here: the structure
 of the oracle's tables (CPU) and the product against the oracle (GPU)."""
 import numpy as np
 import pytest
