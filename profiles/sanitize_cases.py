@@ -94,4 +94,19 @@ assert np.array_equal(e3.encode(img, 80, 5), want) and np.array_equal(d3.decode(
 e3.close()
 d3.close()
 print("ok stripes", flush=True)
+# skewed and saturated content (tests/_content.py): K3 units too long for the staging area (walks on global memory) and
+# K2 slots that overflow in a few segments (band, first frame on a fresh encoder), periodic stream (tiled), bit strings
+# that spill to global memory (binary); the stripe variables above stay set, so K2 and K3 also run stripe by stripe
+import _content as ct  # noqa: E402
+content = [("band", 100, 8, 0, "4:4:4", (1, 1)), ("tiled", 75, 8, 0, "4:4:4", (1, 1)), ("binary", 100, 8, 0, "4:4:4", (1, 1)),
+           ("band", 100, 1, 1, "4:2:0", (2, 2))]
+for kind, q, rst, il, name, samp in content[:2] if quick else content:
+    img = ct.gen(kind, tile=ct.tile_for(samp))
+    want = o.encode(img, q, rst, il, sampling=samp)
+    e4, d4 = g.Encoder(), g.Decoder()
+    assert np.array_equal(e4.encode(img, q, rst, il, subsampling=name), want), (kind, name)
+    assert np.array_equal(d4.decode(want), o.decode(want)), (kind, name)
+    e4.close()
+    d4.close()
+    print("ok content", kind, q, rst, il, name, flush=True)
 print("all sanitizer cases ok")
