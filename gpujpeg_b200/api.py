@@ -97,6 +97,7 @@ def _load():
         "gpujpegx_encoder_get_coefficients": (ci, [vp, vp, cs]),
         "gpujpegx_encoder_get_stream": (C.c_longlong, [vp, vp, cs]),
         "gpujpegx_encoder_run_resident": (ci, [vp, vp, ci]),
+        "gpujpegx_encoder_get_symbol_counts": (ci, [vp, vp]),
         "gpujpegx_decoder_run_resident": (ci, [vp, vp, ci]),
         "gpujpegx_decoder_get_coefficients": (ci, [vp, vp, cs]),
         "gpujpegx_decoder_used_segment_info": (ci, [vp]),
@@ -187,12 +188,15 @@ def _ptr(x):
 class Encoder:
     """gpujpeg_encoder_create / gpujpeg_encoder_encode / gpujpeg_encoder_destroy"""
 
-    def __init__(self, stream=0, pinned_output=False):
+    def __init__(self, stream=0, pinned_output=False, huffman="standard"):
+        """huffman: "standard" (the Annex K tables) or "optimized" (tables fitted to every frame, enc_opt_huffman)"""
         self._h = lib.gpujpeg_encoder_create(C.c_void_p(stream))
         if not self._h:
             raise GpuJpegError("gpujpeg_encoder_create failed (no CUDA device?)")
         if pinned_output:
             self.set_option("enc_opt_out", "enc_out_val_pinned")
+        if huffman != "standard":
+            self.set_option("enc_opt_huffman", huffman)
 
     def set_option(self, key, val):
         if lib.gpujpeg_encoder_set_option(self._h, key.encode(), val.encode()) != 0:
@@ -241,7 +245,8 @@ class Encoder:
         return np.ctypeslib.as_array((C.c_uint8 * size).from_address(addr)).copy()
 
     def run_resident(self, d_raw=None, stage_mask=3):
-        """enqueue the GPU stages only (bit0 K1, bit1 K2) on device-resident data; no copies, no sync"""
+        """enqueue the GPU stages only (bit0 K1, bit3 symbol statistics, bit1 K2) on device-resident data; no copies, no
+        sync"""
         addr = _ptr(d_raw)[0] if d_raw is not None else None
         if lib.gpujpegx_encoder_run_resident(self._h, addr, stage_mask) != 0:
             raise GpuJpegError("gpujpegx_encoder_run_resident failed")
@@ -264,6 +269,14 @@ class Encoder:
             out = np.empty(coefficient_count(width, height, sampling, interleaved), np.int16)
         if lib.gpujpegx_encoder_get_coefficients(self._h, out.ctypes.data, out.size) != 0:
             raise GpuJpegError("gpujpegx_encoder_get_coefficients failed")
+        return out
+
+    def symbol_counts(self):
+        """the last frame's Huffman symbol counts (huffman="optimized", or run_resident with bit 3), uint64
+        [table class][DC 0 / AC 1][symbol]"""
+        out = np.zeros((2, 2, 256), np.uint64)
+        if lib.gpujpegx_encoder_get_symbol_counts(self._h, out.ctypes.data) != 0:
+            raise GpuJpegError("gpujpegx_encoder_get_symbol_counts failed")
         return out
 
     def stats(self):

@@ -48,6 +48,11 @@ struct gpujpeg_encoder {
     struct gj_huff_spec spec[2][2];
     struct gj_dev_enc_tables h_tab;            /* host copy (K1 takes it by value) */
     struct gj_dev_enc_tables* d_tab;           /* device copy (K2 LUTs) */
+    int huff_optimized;                        /* enc_opt_huffman=optimized: tables fitted to every frame */
+    int spec_custom;                           /* spec / LUTs / header hold fitted tables, not Annex K */
+    uint64_t* d_counts;                        /* [2][2][256] symbol counts of the statistics kernel */
+    uint64_t* h_counts;                        /* pinned copy */
+    int counts_valid;                          /* the statistics kernel has run on the current geometry */
 
     /* device buffers */
     uint8_t* d_raw; size_t d_raw_size;
@@ -151,7 +156,8 @@ struct gpujpeg_encoder* gpujpeg_encoder_create(cudaStream_t stream)
     for ( int t = 0; t < 2; t++ )
         gj_enc_lut_build(&e->spec[t][0], &e->spec[t][1], &e->h_tab.lut[t]);
     if ( gj_cuda_malloc((void**)&e->d_tab, sizeof *e->d_tab) || gj_cuda_malloc((void**)&e->d_info, 64) ||
-         gj_cuda_malloc_host((void**)&e->h_info, 64) ) {
+         gj_cuda_malloc_host((void**)&e->h_info, 64) || gj_cuda_malloc((void**)&e->d_counts, GJ_HUFF_COUNTS_BYTES) ||
+         gj_cuda_malloc_host((void**)&e->h_counts, GJ_HUFF_COUNTS_BYTES) ) {
         GJ_ERR("Encoder allocation failed: %s\n", gj_cuda_last_error());
         gpujpeg_encoder_destroy(e);
         return NULL;
@@ -166,6 +172,8 @@ int gpujpeg_encoder_destroy(struct gpujpeg_encoder* e)
     if ( !e ) return -1;
     gj_cuda_free(e->d_tab);
     gj_cuda_free(e->d_info);
+    gj_cuda_free(e->d_counts);
+    if ( e->h_counts ) gj_cuda_free_host(e->h_counts);
     gj_cuda_free(e->d_sos);
     free(e->h_pre);
     free(e->header);
@@ -394,7 +402,8 @@ static int encode_striped(struct gpujpeg_encoder* e, const uint8_t* h_image, int
         const char* v = getenv("GPUJPEG_B200_STRIPES_K2");
         e->k2_parts = !(v && v[0] == '0');
     }
-    const int parts = e->k2_parts && gj_huffman_encode_parts_eligible(&ha);
+    /* (fitted tables are known only when the last stripe has been counted: then K2 runs behind the stripes) */
+    const int parts = e->k2_parts && !e->huff_optimized && gj_huffman_encode_parts_eligible(&ha);
     int segs_done[GJ_MAX_COMP] = {0, 0, 0, 0};
     const int mcu_h = 8 * g->max_vs;                                  /* image rows per MCU row (4:4:4: one block row) */
     const int mcu_rows = (g->bcy + g->max_vs - 1) / g->max_vs;
@@ -477,6 +486,52 @@ static void fill_huff_args(const struct gpujpeg_encoder* e, struct gj_huff_enc_a
     ha->d_info_next = e->d_info + 4 * (e->info_parity ^ 1);
     ha->info_is_zero = e->info_clean;
     ha->d_tables = e->d_tab;
+}
+
+/* the symbol statistics of the frame K1 left in place (enqueued only) */
+static int launch_stats(struct gpujpeg_encoder* e)
+{
+    struct gj_huff_enc_args ha;
+    fill_huff_args(e, &ha);
+    if ( gj_launch_huffman_stats(&ha, e->d_counts, e->stream) ) return -1;
+    e->counts_valid = 1;
+    return 0;
+}
+
+/* enc_opt_huffman=optimized, between K1 and K2: statistics -> (one synchronisation) -> the tables T.81 Annex K.2 fits to them
+ * for the classes the frame's components use (Annex K for an unused class) -> encoder LUTs on the device and the file header.
+ * One table set per class per frame, in the file header, as libjpeg writes baseline streams. */
+static int fit_huffman_tables(struct gpujpeg_encoder* e)
+{
+    const struct gj_geometry* g = &e->geo;
+    if ( launch_stats(e) || gj_cuda_memcpy_d2h_async(e->h_counts, e->d_counts, GJ_HUFF_COUNTS_BYTES, e->stream) ||
+         gj_cuda_stream_sync(e->stream) )
+        return -1;
+    int used[2] = {0, 0};
+    for ( int c = 0; c < g->comp_count; c++ )
+        used[g->lay.comp_tbl[c]] = 1;
+    for ( int t = 0; t < 2; t++ ) {
+        for ( int k = 0; k < 2; k++ ) {
+            if ( used[t] ) gj_huff_spec_optimal(e->h_counts + (t * 2 + k) * 256, &e->spec[t][k]);
+            else gj_huff_spec_default(t, k, &e->spec[t][k]);
+        }
+        gj_enc_lut_build(&e->spec[t][0], &e->spec[t][1], &e->h_tab.lut[t]);
+    }
+    e->spec_custom = 1;
+    /* the DHT segments of fitted tables are longer than Annex K's: up to 256 values each */
+    const size_t need = GJ_HEADER_BASE_CAP + 4 * 256 + gj_exif_tags_bytes(e->extras.exif_tags);
+    if ( need > e->header_cap ) {
+        free(e->header);
+        e->header = (uint8_t*)malloc(need);
+        e->header_cap = e->header ? need : 0;
+        if ( !e->header ) return -1;
+    }
+    e->header_size = gj_write_header(e->header, &e->param, &e->param_image, e->raw_q, e->spec, e->header_type, &e->extras);
+    if ( e->header_size + 64 > g->stream_cap ) {
+        GJ_ERR("The header (%zu bytes) does not fit the stream buffer of a %dx%d image.\n", e->header_size, g->width, g->height);
+        return -1;
+    }
+    return gj_cuda_memcpy_h2d_async(e->d_tab, &e->h_tab, sizeof e->h_tab, e->stream);
 }
 
 /* (re)build everything that depends on geometry [ref: src/gpujpeg_common.c:628-1106] */
@@ -688,6 +743,17 @@ int gpujpeg_encoder_encode(struct gpujpeg_encoder* e, const struct gpujpeg_param
         e->quality = a.quality;
         tables_dirty = 1;
     }
+    /* enc_opt_huffman=standard after fitted tables: back to Annex K (LUTs, header and device copy are rebuilt below) */
+    if ( !e->huff_optimized && e->spec_custom ) {
+        for ( int t = 0; t < 2; t++ ) {
+            for ( int k = 0; k < 2; k++ )
+                gj_huff_spec_default(t, k, &e->spec[t][k]);
+            gj_enc_lut_build(&e->spec[t][0], &e->spec[t][1], &e->h_tab.lut[t]);
+        }
+        e->spec_custom = 0;
+        tables_dirty = 1;
+    }
+    e->counts_valid = 0;
     int geometry_dirty = 0;
     if ( img_changed || !same_param(&e->param, &a) || e->out_is_pinned != e->out_pinned || !e->out ||
          (e->flipped != 0) != e->flip_mode ) {
@@ -837,6 +903,10 @@ int gpujpeg_encoder_encode(struct gpujpeg_encoder* e, const struct gpujpeg_param
     if ( stats && e->timers_ok ) {
         gj_timer_stop(&e->t_pre, e->stream);
         gj_timer_start(&e->t_huff, e->stream);
+    }
+    if ( !k2_done && e->huff_optimized && fit_huffman_tables(e) ) {
+        GJ_ERR("Huffman statistics / table construction failed: %s\n", gj_cuda_last_error());
+        return GPUJPEG_ERROR;
     }
     if ( !k2_done && launch_k2(e) ) {
         GJ_ERR("Huffman encoder launch failed: %s\n", gj_cuda_last_error());
@@ -1034,6 +1104,15 @@ int gpujpeg_encoder_set_option(struct gpujpeg_encoder* encoder, const char* opt,
         encoder->extras_dirty = 1;
         return add_metadata(&encoder->extras.metadata, val);
     }
+    if ( strcmp(opt, GPUJPEG_ENC_OPT_HUFFMAN) == 0 ) {   /* extension: Huffman tables fitted to every frame */
+        if ( strcmp(val, GPUJPEG_ENC_HUFFMAN_VAL_STANDARD) == 0 ) encoder->huff_optimized = 0;
+        else if ( strcmp(val, GPUJPEG_ENC_HUFFMAN_VAL_OPTIMIZED) == 0 ) encoder->huff_optimized = 1;
+        else {
+            GJ_ERR("Unknown Huffman table choice: %s\n", val);
+            return GPUJPEG_ERROR;
+        }
+        return GPUJPEG_NOERR;
+    }
     GJ_ERR("Invalid encoder option: %s!\n", opt);
     return GPUJPEG_ERROR;
 }
@@ -1050,10 +1129,13 @@ void gpujpeg_encoder_print_options(void)
            "] - whether is the input image should be vertically flipped (prior encode)\n");
     printf("\t" GPUJPEG_ENC_OPT_CHANNEL_REMAP "=XYZ[W] - input channel mapping, eg. '210F' for GBRX,\n"
            "\t\t'210' for GBR; special placeholders 'F' and 'Z' to set a channel to all-ones or all-zeros\n");
+    printf("\t" GPUJPEG_ENC_OPT_HUFFMAN "=[" GPUJPEG_ENC_HUFFMAN_VAL_STANDARD "|" GPUJPEG_ENC_HUFFMAN_VAL_OPTIMIZED
+           "] - Huffman tables of T.81 Annex K (default) or fitted to every frame\n");
 }
 
 /* ---- extension: re-run the GPU stages of the last configured frame on device-resident data ----
- * stage_mask bit 0 = K1 (colour+FDCT+quant), bit 1 = K2 (Huffman encode + scan assembly).  Nothing is
+ * stage_mask bit 0 = K1 (colour+FDCT+quant), bit 3 = the symbol statistics of enc_opt_huffman=optimized (kernel alone),
+ * bit 1 = K2 (Huffman encode + scan assembly, with the tables the last gpujpeg_encoder_encode chose).  Nothing is
  * copied to or from the host and nothing is synchronised: the caller times the stream with CUDA events.
  * d_raw == NULL re-uses the device copy of the last host image.  Used by bench.py for the
  * "inputs already resident in HBM" number and for per-stage roofline timing. */
@@ -1063,7 +1145,18 @@ GPUJPEG_API int gpujpegx_encoder_run_resident(struct gpujpeg_encoder* e, const u
     if ( !d_raw ) d_raw = e->d_raw;
     if ( !d_raw ) return -1;
     if ( (stage_mask & 1) && launch_k1(e, d_raw) ) return -1;
+    if ( (stage_mask & 8) && launch_stats(e) ) return -1;
     if ( (stage_mask & 2) && launch_k2(e) ) return -1;
+    return 0;
+}
+
+/* ---- extension used by the parity tests: the symbol counts the statistics kernel found in the last frame ---- */
+GPUJPEG_API int gpujpegx_encoder_get_symbol_counts(struct gpujpeg_encoder* e, uint64_t out[2][2][256])
+{
+    if ( !e || !e->initialised || !e->counts_valid || !out ) return -1;
+    if ( gj_cuda_memcpy_d2h_async(e->h_counts, e->d_counts, GJ_HUFF_COUNTS_BYTES, e->stream) || gj_cuda_stream_sync(e->stream) )
+        return -1;
+    memcpy(out, e->h_counts, GJ_HUFF_COUNTS_BYTES);
     return 0;
 }
 

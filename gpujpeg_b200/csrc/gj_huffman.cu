@@ -768,6 +768,118 @@ k_huff_place(const uint8_t* __restrict__ tmp, size_t slot_stride, const uint32_t
     }
 }
 
+/* ------------------------------------------------------------------------------------------- */
+/* k_huff_stats: the symbol histogram of a frame for enc_opt_huffman=optimized -- every DC category and every AC run/size
+ * symbol (ZRL and EOB included) per table class, counted exactly as K2 emits them.  One THREAD per block in scan order, so
+ * the work does not depend on the restart interval (a warp per segment, as in K2, would put a whole scan on one warp at
+ * restart_interval = 0): the thread finds its segment and its place j in it by arithmetic, takes the DC predictor from the
+ * block j - pd of the same segment (0 when j < pd) and walks its non-zero mask, reading only the non-zero values.
+ * Counting: equal symbols of a warp are merged (__match_any_sync) into ONE shared atomic -- uniform content sends all 32
+ * lanes to the same bin --, ZRL and EOB are summed in registers; a CTA adds each non-empty bin once to the 64-bit counters. */
+constexpr int HS_THREADS = 256;
+constexpr int HS_BINS = 2 * 2 * 256;   // [table class][DC 0 / AC 1][symbol]
+constexpr int HS_CTAS_PER_SM = 8;
+
+__device__ __forceinline__ void hs_add(uint32_t* hist, int key, bool valid, int lane)
+{
+    const unsigned act = __ballot_sync(FULL, valid);
+    if ( valid ) {
+        const unsigned peers = __match_any_sync(act, key);
+        if ( __ffs((int)peers) - 1 == lane ) atomicAdd(&hist[key], (uint32_t)__popc(peers));
+    }
+}
+
+__global__ void __launch_bounds__(HS_THREADS)
+k_huff_stats(const int16_t* __restrict__ coef, const uint64_t* __restrict__ nzmask, const __grid_constant__ gj_scan_layout lay,
+             int seg_mcu, int total_blocks, unsigned long long* __restrict__ counts)
+{
+    gj_pdl_wait();
+    __shared__ uint32_t s_hist[HS_BINS];
+    /* the block's first 16 coefficients (one 32-byte sector: nearly all non-zeros of photographic content), fetched with
+     * the mask so that the walk below waits on a load only for the high frequencies (the 48-byte stride as in K2) */
+    __shared__ __align__(16) uint32_t s_head[HS_THREADS * HE_HEAD];
+    for ( int i = threadIdx.x; i < HS_BINS; i += HS_THREADS )
+        s_hist[i] = 0;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const int segblk = seg_mcu * lay.bpm;
+    uint32_t* head = s_head + threadIdx.x * HE_HEAD;
+    const int16_t* head16 = reinterpret_cast<const int16_t*>(head);
+    uint32_t zrl0 = 0, zrl1 = 0, eob0 = 0, eob1 = 0;
+    /* the loop bound is uniform over the warp: every lane takes part in the warp-wide merges below */
+    for ( int t0 = blockIdx.x * HS_THREADS + (threadIdx.x & ~31); t0 < total_blocks; t0 += gridDim.x * HS_THREADS ) {
+        const int t = t0 + lane;
+        const bool active = t < total_blocks;
+        int tbl = 0, dcat = 0;
+        uint64_t nz = 0;
+        const int16_t* blk = coef;
+        if ( active ) {
+            int scan = 0, base = 0;
+            for ( ; scan + 1 < lay.scan_count; scan++ ) {
+                const int n = lay.scan_mcus[scan] * lay.bpm;
+                if ( t < base + n ) break;
+                base += n;
+            }
+            const int r = t - base, s = r / segblk, j = r - s * segblk;
+            size_t bi;
+            int comp, pd;
+            segment_block(lay, scan, s * seg_mcu, j, bi, comp, pd);
+            tbl = lay.comp_tbl[comp];
+            /* DC predictor: previous block of the same component inside the segment, 0 at its start (as K2) */
+            int pred = 0;
+            if ( j >= pd ) {
+                size_t bp;
+                int cp, pp;
+                segment_block(lay, scan, s * seg_mcu, j - pd, bp, cp, pp);
+                pred = __ldg(coef + bp * 64);
+            }
+            blk = coef + bi * 64;
+            nz = __ldg(nzmask + bi);
+            const uint4 ha = __ldg(reinterpret_cast<const uint4*>(blk)), hb = __ldg(reinterpret_cast<const uint4*>(blk) + 1);
+            reinterpret_cast<uint4*>(head)[0] = ha;   // only this thread reads its head
+            reinterpret_cast<uint4*>(head)[1] = hb;
+            dcat = gj_category((int)(short)(ha.x & 0xFFFFu) - pred);
+        }
+        hs_add(s_hist, tbl * 512 + dcat, active, lane);
+        uint64_t m = nz & ~1ull;
+        int last = 0;
+        while ( __any_sync(FULL, m != 0) ) {
+            const bool has = m != 0;
+            int key = 0;
+            if ( has ) {
+                const int k = __ffsll((long long)m) - 1;
+                m &= m - 1;
+                const int run = k - last - 1;
+                last = k;
+                if ( tbl ) zrl1 += (uint32_t)(run >> 4);
+                else zrl0 += (uint32_t)(run >> 4);
+                const int v = k < 16 ? (int)head16[k] : (int)__ldg(blk + k);
+                key = tbl * 512 + 256 + ((run & 15) << 4) + gj_category(v);
+            }
+            hs_add(s_hist, key, has, lane);
+        }
+        if ( active && last < 63 ) {
+            if ( tbl ) eob1++;
+            else eob0++;
+        }
+    }
+    zrl0 = __reduce_add_sync(FULL, zrl0);
+    zrl1 = __reduce_add_sync(FULL, zrl1);
+    eob0 = __reduce_add_sync(FULL, eob0);
+    eob1 = __reduce_add_sync(FULL, eob1);
+    if ( lane == 0 ) {
+        if ( zrl0 ) atomicAdd(&s_hist[256 + 0xF0], zrl0);
+        if ( zrl1 ) atomicAdd(&s_hist[512 + 256 + 0xF0], zrl1);
+        if ( eob0 ) atomicAdd(&s_hist[256], eob0);
+        if ( eob1 ) atomicAdd(&s_hist[512 + 256], eob1);
+    }
+    __syncthreads();
+    for ( int i = threadIdx.x; i < HS_BINS; i += HS_THREADS ) {
+        const uint32_t v = s_hist[i];
+        if ( v ) atomicAdd(counts + i, (unsigned long long)v);
+    }
+}
+
 /* =========================================================================================== */
 /* decoder                                                                                       */
 
@@ -1148,6 +1260,20 @@ extern "C" int gj_launch_huffman_encode(const struct gj_huff_enc_args* a, gj_str
         if ( cudaGetLastError() != cudaSuccess ) return -1;
     }
     return gj_launch_huffman_place(a, stream);
+}
+
+extern "C" int gj_launch_huffman_stats(const struct gj_huff_enc_args* a, uint64_t* d_counts, gj_stream_t stream)
+{
+    int total = 0;
+    for ( int k = 0; k < a->lay.scan_count; k++ )
+        total += a->lay.scan_mcus[k] * a->lay.bpm;
+    if ( total <= 0 || a->seg_mcu <= 0 ) return -1;
+    if ( cudaMemsetAsync(d_counts, 0, HS_BINS * sizeof(uint64_t), stream) != cudaSuccess ) return -1;
+    /* a few CTAs per SM walk the frame in strides: each adds its bins to the global counters once */
+    const int ctas = min((total + HS_THREADS - 1) / HS_THREADS, HS_CTAS_PER_SM * gj_cuda_sm_count());
+    gj_launch_pdl(k_huff_stats, dim3(ctas), dim3(HS_THREADS), 0, stream, a->d_coef, a->d_nzmask, a->lay, a->seg_mcu, total,
+                  reinterpret_cast<unsigned long long*>(d_counts));
+    return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
 extern "C" int gj_huffman_decode_sync_eligible(const struct gj_huff_dec_args* a);

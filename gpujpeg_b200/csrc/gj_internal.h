@@ -46,6 +46,8 @@ struct gj_huff_spec {
     int nvals;
 };
 void gj_huff_spec_default(int cls /*0 lum,1 chroma*/, int kind /*0 DC,1 AC*/, struct gj_huff_spec* spec);
+/* the table T.81 Annex K.2 fits to a symbol histogram, byte for byte what libjpeg's optimize_coding writes (enc_opt_huffman) */
+void gj_huff_spec_optimal(const uint64_t freq[256], struct gj_huff_spec* spec);
 
 /* quantisation: raw zig-zag u8 table for a quality [ref: src/gpujpeg_table.c:83-99] */
 void gj_quant_raw(int cls, int quality, uint8_t raw_zz[64]);
@@ -335,6 +337,10 @@ int gj_huffman_encode_parts_eligible(const struct gj_huff_enc_args* a);
 int gj_launch_huffman_encode_part(const struct gj_huff_enc_args* a, int first, const int lo[GJ_MAX_COMP], const int n[GJ_MAX_COMP],
                                   gj_stream_t stream);
 int gj_launch_huffman_place(const struct gj_huff_enc_args* a, gj_stream_t stream);
+/* symbol statistics of the frame K1 left in place, exactly as K2 would emit the symbols: d_counts[table class][DC 0 / AC 1]
+ * [symbol] (2 x 2 x 256 64-bit counters, cleared by the launch) -- the input of enc_opt_huffman=optimized */
+#define GJ_HUFF_COUNTS_BYTES (2 * 2 * 256 * sizeof(uint64_t))
+int gj_launch_huffman_stats(const struct gj_huff_enc_args* a, uint64_t* d_counts, gj_stream_t stream);
 
 /* K3: Huffman-decode every restart segment into zig-zag coefficients
  * [replaces ref: src/gpujpeg_huffman_gpu_decoder.cu:663-746] */

@@ -71,6 +71,76 @@ void gj_huff_spec_default(int cls, int kind, struct gj_huff_spec* spec)
     }
 }
 
+/* Huffman table fitted to a histogram: T.81 Annex K.2 with the choices libjpeg makes (jchuff.c, jpeg_gen_optimal_table), so
+ * that the same counts give the same DHT bytes as libjpeg's optimize_coding:
+ *   K.1  a reserved symbol 256 with count 1 keeps the all-ones code unused; the two smallest non-zero counts are merged
+ *        until one is left, and among equal counts the HIGHER symbol number is taken (a `<=` scan upwards);
+ *   K.2/K.3  code sizes counted into BITS, then limited to 16 bits; the reserved code leaves the longest length in use;
+ *   K.4  HUFFVAL in the order of the unadjusted code sizes, then of the symbol values.
+ * Counts are 64-bit and compared without libjpeg's 10^9 sentinel.  A tree of 257 leaves is at most 256 deep. */
+#define GJ_HUFF_MAX_DEPTH 256
+void gj_huff_spec_optimal(const uint64_t freq_in[256], struct gj_huff_spec* spec)
+{
+    uint64_t freq[257];
+    int others[257], codesize[257];
+    int bits[GJ_HUFF_MAX_DEPTH + 1];
+    memset(spec, 0, sizeof *spec);
+    memset(bits, 0, sizeof bits);
+    for ( int i = 0; i < 256; i++ )
+        freq[i] = freq_in[i];
+    freq[256] = 1;
+    for ( int i = 0; i <= 256; i++ ) {
+        others[i] = -1;
+        codesize[i] = 0;
+    }
+    for ( ;; ) {
+        int c1 = -1, c2 = -1;
+        for ( int i = 0; i <= 256; i++ )
+            if ( freq[i] && (c1 < 0 || freq[i] <= freq[c1]) ) c1 = i;
+        for ( int i = 0; i <= 256; i++ )
+            if ( freq[i] && i != c1 && (c2 < 0 || freq[i] <= freq[c2]) ) c2 = i;
+        if ( c2 < 0 ) break;
+        freq[c1] += freq[c2];
+        freq[c2] = 0;
+        codesize[c1]++;
+        while ( others[c1] >= 0 ) {
+            c1 = others[c1];
+            codesize[c1]++;
+        }
+        others[c1] = c2;
+        codesize[c2]++;
+        while ( others[c2] >= 0 ) {
+            c2 = others[c2];
+            codesize[c2]++;
+        }
+    }
+    for ( int i = 0; i <= 256; i++ )
+        if ( codesize[i] ) bits[codesize[i]]++;
+    /* Figure K.3: a pair of codes of length i becomes one of length i - 1 and one of length j + 1 */
+    int i = GJ_HUFF_MAX_DEPTH;
+    for ( ; i > 16; i-- ) {
+        while ( bits[i] > 0 ) {
+            int j = i - 2;
+            while ( bits[j] == 0 )
+                j--;
+            bits[i] -= 2;
+            bits[i - 1]++;
+            bits[j + 1] += 2;
+            bits[j]--;
+        }
+    }
+    while ( i > 0 && bits[i] == 0 )
+        i--;
+    if ( i > 0 ) bits[i]--;   /* the reserved code */
+    for ( int l = 1; l <= 16; l++ )
+        spec->bits[l] = (uint8_t)bits[l];
+    int p = 0;
+    for ( int l = 1; l <= GJ_HUFF_MAX_DEPTH; l++ )
+        for ( int s = 0; s < 256; s++ )
+            if ( codesize[s] == l ) spec->vals[p++] = (uint8_t)s;
+    spec->nvals = p;
+}
+
 /* [ref: src/gpujpeg_table.c:83-99] libjpeg-style quality scaling, clamp to [1,255] */
 void gj_quant_raw(int cls, int quality, uint8_t raw_zz[64])
 {

@@ -377,6 +377,12 @@ GPUJPEG_API int gpujpeg_encoder_suggest_restart_interval(const struct gpujpeg_im
 #define GPUJPEG_ENC_OPT_EXIF_TAG "enc_exif_tag"
 #define GPUJPEG_ENC_OPT_METADATA "enc_metadata"
 #define GPUJPEG_ENC_OPT_CHANNEL_REMAP "enc_opt_channel_remap"
+/* extension: which Huffman tables the encoder writes.  "standard" (default): the example tables of T.81 Annex K, as the
+ * reference; "optimized": tables fitted to every frame (T.81 Annex K.2, libjpeg's optimize_coding), counted on the GPU --
+ * smaller files for one more host round trip per frame */
+#define GPUJPEG_ENC_OPT_HUFFMAN "enc_opt_huffman"
+#define GPUJPEG_ENC_HUFFMAN_VAL_STANDARD "standard"
+#define GPUJPEG_ENC_HUFFMAN_VAL_OPTIMIZED "optimized"
 GPUJPEG_API int gpujpeg_encoder_set_option(struct gpujpeg_encoder* encoder, const char* opt, const char* val);
 GPUJPEG_API void gpujpeg_encoder_print_options(void);
 GPUJPEG_API int gpujpeg_encoder_destroy(struct gpujpeg_encoder* encoder);

@@ -20,9 +20,13 @@ extern "C" {
 #endif
 
 /* ---- resident re-runs (no copies, no synchronisation; the caller times the coder's stream) ---- */
-/* stage_mask: bit 0 = K1 (colour + FDCT + quantisation), bit 1 = K2 (Huffman encode + scan assembly); d_raw == NULL
+/* stage_mask: bit 0 = K1 (colour + FDCT + quantisation), bit 3 = the symbol statistics of enc_opt_huffman=optimized alone,
+ * bit 1 = K2 (Huffman encode + scan assembly, with the tables the last gpujpeg_encoder_encode chose); d_raw == NULL
  * re-uses the device copy of the last host image */
 GPUJPEG_API int gpujpegx_encoder_run_resident(struct gpujpeg_encoder* encoder, const uint8_t* d_raw, int stage_mask);
+/* the symbol counts of the last frame's statistics (enc_opt_huffman=optimized, or a resident run with bit 3), indexed
+ * [table class][DC 0 / AC 1][symbol] (parity tests); -1 when no statistics have run since the last encode */
+GPUJPEG_API int gpujpegx_encoder_get_symbol_counts(struct gpujpeg_encoder* encoder, uint64_t out[2][2][256]);
 /* stage_mask: bit 2 = K0 (marker list + clean stream from the JPEG bytes on the device), bit 0 = K3 (Huffman decode),
  * bit 1 = K4 (dequantisation + IDCT + colour); d_out == NULL writes into the decoder's own buffer */
 GPUJPEG_API int gpujpegx_decoder_run_resident(struct gpujpeg_decoder* decoder, uint8_t* d_out, int stage_mask);
