@@ -453,6 +453,64 @@ static size_t scan_end(const uint8_t* d, size_t b, size_t size)
     return size;
 }
 
+/* The scan parameters of a progressive frame (T.81 G.1.1.1): a DC scan (Ss = 0, Se = 0) may interleave components, an AC
+ * scan (0 < Ss <= Se <= 63) codes one; a first scan has Ah = 0, a refinement Al = Ah - 1; Al <= 13.  Per component and
+ * coefficient the scans must form one successive-approximation sequence (a first scan, then refinements one bit at a
+ * time), and no AC scan may come before the component's first DC scan.  Also latches the quantisation table of a
+ * component at its first scan and records the Huffman tables in force. */
+static int progressive_scan_check(struct gj_stream* s, struct gj_scan_info* sc)
+{
+    if ( sc->ss == 0 ? sc->se != 0 : (sc->se < sc->ss || sc->se > 63 || sc->ncomp != 1) ) {
+        GJ_ERR("Invalid progressive scan: Ss %d, Se %d with %d component(s)!\n", sc->ss, sc->se, sc->ncomp);
+        return -1;
+    }
+    if ( (sc->ah != 0 && sc->al != sc->ah - 1) || sc->al > 13 ) {
+        GJ_ERR("Invalid progressive scan: Ah %d, Al %d!\n", sc->ah, sc->al);
+        return -1;
+    }
+    for ( int k = 0; k < sc->ncomp; k++ ) {
+        const int c = sc->comp[k];
+        uint8_t* bits = s->coef_bits[c];
+        if ( sc->ss > 0 && bits[0] == 0 ) {
+            GJ_ERR("Invalid progressive scan: AC scan of component %d before its first DC scan!\n", c);
+            return -1;
+        }
+        for ( int i = sc->ss; i <= sc->se; i++ ) {
+            if ( bits[i] != (sc->ah == 0 ? 0 : sc->ah + 1) ) {
+                GJ_ERR("Invalid progressive scan: coefficient %d of component %d refined with Ah %d after %s!\n", i, c, sc->ah,
+                       bits[i] ? "another bit position" : "no first scan");
+                return -1;
+            }
+            bits[i] = (uint8_t)(sc->al + 1);
+        }
+        if ( !s->have_comp_qt[c] ) {   /* the table is latched at the component's first scan, as libjpeg does */
+            if ( !s->have_qt[s->comp_tq[c]] ) {
+                GJ_ERR("Quantization table %d is missing!\n", s->comp_tq[c]);
+                return -1;
+            }
+            memcpy(s->comp_qt[c], s->qt[s->comp_tq[c]], 64);
+            s->have_comp_qt[c] = 1;
+        }
+        const int dc_first = sc->ss == 0 && sc->ah == 0, ac = sc->ss > 0;
+        sc->huff_at[k] = dc_first && s->have_huff[0][sc->td[k]] ? s->huff_at[0][sc->td[k]]
+                         : ac && s->have_huff[1][sc->ta[k]]     ? s->huff_at[1][sc->ta[k]]
+                                                                : 0;
+    }
+    return 0;
+}
+
+void gj_huff_spec_at(const uint8_t* d, size_t at, struct gj_huff_spec* h)
+{
+    memset(h, 0, sizeof *h);
+    int cnt = 0;
+    for ( int k = 1; k <= 16; k++ ) {
+        h->bits[k] = d[at + (size_t)k];
+        cnt += d[at + (size_t)k];
+    }
+    memcpy(h->vals, d + at + 17, (size_t)cnt);
+    h->nvals = cnt;
+}
+
 /* Walks marker segments starting at *pos.  Returns 1 when an SOS header was parsed (a new entry in
  * s->scan with .begin = first entropy-coded byte, *pos = .begin), 0 at EOI or end of data, -1 on error.
  * Never looks at entropy-coded data. */
@@ -576,10 +634,12 @@ int gj_reader_walk(const uint8_t* d, size_t size, size_t* pos, struct gj_stream*
                 break;
             }
             case 0xC0: /* [ref: src/gpujpeg_reader.c:806-886] */
+            case 0xC2: /* progressive, Huffman: the same frame header (T.81 B.2.2) */
                 if ( n < 6 || b[0] != 8 ) {
-                    GJ_ERR("SOF0 marker precision should be 8 but %d was presented!\n", n >= 1 ? b[0] : -1);
+                    GJ_ERR("SOF%d marker precision should be 8 but %d was presented!\n", m - 0xC0, n >= 1 ? b[0] : -1);
                     return -1;
                 }
+                s->progressive = m == 0xC2;
                 s->height = r16(b + 1);
                 s->width = r16(b + 3);
                 s->comp_count = b[5];
@@ -594,9 +654,9 @@ int gj_reader_walk(const uint8_t* d, size_t size, size_t* pos, struct gj_stream*
                     if ( s->comp_tq[c] > 3 ) return -1;
                 }
                 break;
-            case 0xC1: case 0xC2: case 0xC3: case 0xC5: case 0xC6: case 0xC7:
+            case 0xC1: case 0xC3: case 0xC5: case 0xC6: case 0xC7:
             case 0xC9: case 0xCA: case 0xCB: case 0xCD: case 0xCE: case 0xCF:
-                GJ_ERR("Unsupported JPEG process (SOF marker 0x%X): only baseline is supported!\n", m);
+                GJ_ERR("Unsupported JPEG process (SOF marker 0x%X): only baseline and Huffman progressive are supported!\n", m);
                 return -1;
             case 0xC4: { /* [ref: src/gpujpeg_reader.c:920-986] */
                 int off = 0;
@@ -621,6 +681,7 @@ int gj_reader_walk(const uint8_t* d, size_t size, size_t* pos, struct gj_stream*
                     memcpy(h->vals, b + off + 17, (size_t)cnt);
                     h->nvals = cnt;
                     s->have_huff[tc][th] = 1;
+                    s->huff_at[tc][th] = (size_t)(b - d) + (size_t)off;
                     off += 17 + cnt;
                 }
                 break;
@@ -634,8 +695,9 @@ int gj_reader_walk(const uint8_t* d, size_t size, size_t* pos, struct gj_stream*
                     GJ_ERR("SOS marker before SOF0!\n");
                     return -1;
                 }
-                if ( s->scan_count >= GJ_MAX_COMP ) {
-                    GJ_ERR("Too many scans!\n");
+                if ( s->scan_count >= (s->progressive ? GJ_MAX_SCANS : GJ_MAX_COMP) ) {
+                    if ( s->progressive ) GJ_ERR("Too many scans (a progressive frame may have at most %d)!\n", GJ_MAX_SCANS);
+                    else GJ_ERR("Too many scans!\n");
                     return -1;
                 }
                 if ( s->scan_count == 0 ) s->header_size = i;
@@ -643,7 +705,7 @@ int gj_reader_walk(const uint8_t* d, size_t size, size_t* pos, struct gj_stream*
                     GJ_ERR("SOS marker is too short (%d bytes)!\n", len);
                     return -1;
                 }
-                s->seginfo[s->scan_count] = s->seginfo_pending;   /* the table belongs to the scan that follows it */
+                if ( s->scan_count < GJ_MAX_COMP ) s->seginfo[s->scan_count] = s->seginfo_pending;   /* the table belongs to the scan that follows it */
                 memset(&s->seginfo_pending, 0, sizeof s->seginfo_pending);
                 struct gj_scan_info* sc = &s->scan[s->scan_count++];
                 memset(sc, 0, sizeof *sc);
@@ -662,6 +724,11 @@ int gj_reader_walk(const uint8_t* d, size_t size, size_t* pos, struct gj_stream*
                     sc->ta[k] = b[2 + 2 * k] & 15;
                     if ( sc->td[k] > 3 || sc->ta[k] > 3 ) return -1;
                 }
+                sc->ss = b[1 + 2 * sc->ncomp];
+                sc->se = b[2 + 2 * sc->ncomp];
+                sc->ah = b[3 + 2 * sc->ncomp] >> 4;
+                sc->al = b[3 + 2 * sc->ncomp] & 15;
+                if ( s->progressive && progressive_scan_check(s, sc) ) return -1;
                 sc->begin = i + 2 + (size_t)len;
                 sc->end = sc->begin;
                 *pos = sc->begin;
@@ -784,4 +851,57 @@ int gj_reader_split(const uint8_t* d, struct gj_stream* s, uint32_t* seg_off, ui
         sc->segment_count = n - sc->first_segment;
     }
     return n;
+}
+
+/* Scan k of a progressive frame on the frame's geometry (T.81 A.2): an interleaved (DC) scan codes the MCUs of the frame,
+ * each with hs x vs blocks of every component it names; a non-interleaved scan codes the component's own
+ * ceil(w_c/8) x ceil(h_c/8) blocks -- the blocks of an MCU-padded plane that lie beyond them are only reached by DC
+ * scans and keep AC = 0, as in libjpeg. */
+int gj_prog_scan_init(const struct gj_geometry* g, const struct gj_stream* s, int k, int restart_interval, struct gj_prog_scan* out)
+{
+    const struct gj_scan_info* sc = &s->scan[k];
+    memset(out, 0, sizeof *out);
+    out->ss = sc->ss;
+    out->se = sc->se;
+    out->ah = sc->ah;
+    out->al = sc->al;
+    out->kind = sc->ss == 0 ? (sc->ah ? GJ_PROG_DC_REFINE : GJ_PROG_DC_FIRST) : (sc->ah ? GJ_PROG_AC_REFINE : GJ_PROG_AC_FIRST);
+    out->ncomp = sc->ncomp;
+    for ( int i = 0; i < sc->ncomp; i++ ) {
+        const int c = sc->comp[i];
+        if ( c < 0 || c >= g->comp_count || (i > 0 && c <= sc->comp[i - 1]) ) return -1;   /* frame order (T.81 B.2.3) */
+        const struct gj_comp_geo* cg = &g->comp[c];
+        out->blk_off[i] = cg->blk_off;
+        out->bcx[i] = cg->bcx;
+        out->nblk[i] = cg->nblk;
+        out->hs[i] = cg->hs;
+        out->vs[i] = cg->vs;
+    }
+    if ( sc->ncomp > 1 ) {
+        if ( !g->interleaved ) return -1;
+        int n = 0;
+        for ( int i = 0; i < sc->ncomp; i++ )
+            for ( int y = 0; y < out->vs[i]; y++ )
+                for ( int x = 0; x < out->hs[i]; x++, n++ ) {
+                    if ( n >= GJ_MAX_MCU_BLOCKS ) return -1;
+                    out->idx_ci[n] = (uint8_t)i;
+                    out->idx_dx[n] = (uint8_t)x;
+                    out->idx_dy[n] = (uint8_t)y;
+                }
+        out->bpm = n;
+        out->units_x = (g->data_width + 8 * g->max_hs - 1) / (8 * g->max_hs);
+        out->units = out->units_x * ((g->data_height + 8 * g->max_vs - 1) / (8 * g->max_vs));
+    }
+    else {
+        const struct gj_comp_geo* cg = &g->comp[sc->comp[0]];
+        out->bpm = 1;
+        out->units_x = (cg->width + 7) / 8;
+        out->units = out->units_x * ((cg->height + 7) / 8);
+        out->idx_ci[0] = 0;
+        if ( out->units_x > cg->bcx || out->units > cg->nblk ) return -1;
+    }
+    if ( out->units <= 0 ) return -1;
+    out->seg_units = restart_interval > 0 ? restart_interval : out->units;
+    out->seg_count = (out->units + out->seg_units - 1) / out->seg_units;
+    return 0;
 }

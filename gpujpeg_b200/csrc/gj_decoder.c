@@ -16,7 +16,8 @@
  *     D2H pixels (unless a device output was requested)
  *
  * Supported: baseline 8-bit YCbCr-JPEG or grey streams, 1 or 3 components, 4:4:4 / 4:2:2 / 4:2:0 / 4:4:0, interleaved or
- * not, any restart interval (or none), any DHT/DQT tables with ids 0..3; output negotiated in choose_output():
+ * not, any restart interval (or none), any DHT/DQT tables with ids 0..3; progressive (SOF2, Huffman) frames of the same
+ * samplings through decode_progressive (one GPU thread per restart segment of a scan); output negotiated in choose_output():
  * GPUJPEG_RGB 444-u8-p012 through the fused kernel, the stream's own samples in a matching pixel format straight from
  * the IDCT, every other pixel format x colour space combination through the generic pass.
  */
@@ -91,6 +92,13 @@ struct gpujpeg_decoder {
     size_t last_ecs_begin; uint32_t last_list_cap;
     int last_tq[GJ_MAX_COMP];
     int last_valid;
+
+    /* progressive frames (decode_progressive): the last frame's scans and launch arguments, every scan's Huffman tables */
+    int last_progressive;
+    struct gj_prog_args last_prog;
+    struct gj_prog_scan* prog_scans;   /* [GJ_MAX_SCANS] */
+    struct gj_dec_lut* h_prog_luts;    /* [GJ_MAX_SCANS * GJ_MAX_COMP] */
+    struct gj_dec_lut* d_prog_luts;
 };
 
 /* ---- output descriptor helpers [ref: src/gpujpeg_decoder.c:44-92] ---- */
@@ -183,6 +191,9 @@ int gpujpeg_decoder_destroy(struct gpujpeg_decoder* d)
     gj_cuda_free(d->d_planes);
     gj_cuda_free(d->d_raw);
     gj_cuda_free_host(d->h_raw);
+    gj_cuda_free(d->d_prog_luts);
+    free(d->prog_scans);
+    free(d->h_prog_luts);
     if ( d->copy_stream ) gj_cuda_stream_destroy(d->copy_stream);
     gj_cuda_event_destroy(d->ev_done);
     for ( int i = 0; i < GJ_STRIPES; i++ )
@@ -623,6 +634,348 @@ static int split_by_segment_info(struct gpujpeg_decoder* d, const uint8_t* image
     return 1;
 }
 
+/* K0 on the uploaded file, its report back to the host, and the host's part of the marker walk: per scan from the report
+ * alone (no second kernel, no walk over the entropy-coded bytes) where it ends, how many markers lie in front of it, where its
+ * clean bytes start; the marker segments between scans are read by length (gj_reader_walk), so that st / pos / adobe end at
+ * the end of the stream.  The rank arrays have room for every scan the reader accepts for the frame's process. */
+static int k0_scan_extents(struct gpujpeg_decoder* d, const uint8_t* image, size_t image_size, size_t ecs_begin, uint32_t list_cap,
+                           struct gj_stream* st, size_t* pos, int* adobe, uint32_t* first_rank, uint32_t* end_rank, uint32_t* scan_cbegin)
+{
+    const struct gj_geometry* g = &d->geo;
+    /* d_mk: [0] total markers, [1] non-RST markers, [2] list overflow, [3] restart sequence error (K3), [5] clean bytes,
+     *       [8..] {rank, position, code, clean position} of the non-RST markers */
+    if ( gj_launch_marker_scan(d->d_file, ecs_begin, image_size, d->d_cta, d->d_list_pos, d->d_list_code, d->d_list_cpos,
+                               list_cap, d->d_clean, d->d_mk, d->d_mk + 8, GJ_MK_OTHER_CAP, d->stream) ||
+         gj_cuda_memcpy_d2h_async(d->h_mk, d->d_mk, GJ_MK_WORDS * 4, d->stream) ||
+         gj_cuda_stream_sync(d->stream) ) {
+        GJ_ERR("Marker scan failed: %s\n", gj_cuda_last_error());
+        return -1;
+    }
+
+    /* ---- host reader, part 2: scan extents from the marker list, marker segments between scans by length ---- */
+    const uint32_t n_other = d->h_mk[1];
+    if ( n_other == 0 || n_other > GJ_MK_OTHER_CAP ) {
+        GJ_ERR("JPEG stream has %u restart markers / %u other markers in its scan data, expected %d restart segments "
+               "for a %dx%d image with restart interval %d!\n", d->h_mk[0], n_other, g->seg_count, st->width, st->height,
+               st->restart_interval);
+        return -1;
+    }
+    uint32_t* other = d->h_mk + 8; /* insertion sort by position: a handful of entries */
+    for ( uint32_t i = 1; i < n_other; i++ ) {
+        uint32_t t[4] = {other[4 * i], other[4 * i + 1], other[4 * i + 2], other[4 * i + 3]};
+        uint32_t j = i;
+        while ( j > 0 && other[4 * (j - 1) + 1] > t[1] ) {
+            memcpy(other + 4 * j, other + 4 * (j - 1), 16);
+            j--;
+        }
+        memcpy(other + 4 * j, t, 16);
+    }
+    /* per scan, from the marker report alone (no second kernel, no walk over the entropy-coded bytes): where it ends,
+     * how many markers lie in front of it, how many restart markers it holds, where its clean bytes start */
+    for ( int k = 0; k < st->scan_count; k++ ) {
+        /* a scan ends at the first marker that is not RSTn: inside entropy-coded data that test is exact */
+        size_t e1 = 0;
+        int last_before = -1;
+        for ( uint32_t i = 0; i < n_other; i++ ) {
+            if ( other[4 * i + 1] >= st->scan[k].begin ) {
+                e1 = other[4 * i + 1];
+                end_rank[k] = other[4 * i];
+                break;
+            }
+            last_before = (int)i;
+        }
+        if ( last_before >= 0 ) {
+            /* the last marker in front of the scan (its SOS): everything up to the scan's first byte that K0 kept
+             * belongs to the clean stream too -- the same keep rule, applied to the few header bytes */
+            const uint32_t* m = other + 4 * last_before;
+            first_rank[k] = m[0] + 1;
+            uint32_t c = m[3];
+            if ( st->scan[k].begin - m[1] > 4096 ) {
+                GJ_ERR("Unsupported scan structure (no marker in front of scan %d).\n", k);
+                return -1;
+            }
+            for ( size_t q = (size_t)m[1] + 2; q < st->scan[k].begin; q++ ) {
+                const int b0 = image[q], b1 = q + 1 < image_size ? image[q + 1] : 0, prev = image[q - 1];
+                if ( !((b0 == 0xFF && b1 != 0) || (prev == 0xFF && b0 != 0xFF)) ) c++;
+            }
+            scan_cbegin[k] = c;
+        }
+        if ( e1 == 0 ) {
+            GJ_ERR("JPEG data unexpected ended while reading SOS marker!\n");
+            return -1;
+        }
+        st->scan[k].end = e1;
+        *pos = e1;
+        const int r = gj_reader_walk(image, image_size, pos, st, adobe);
+        if ( r < 0 ) return -1;
+        if ( r == 0 ) break; /* EOI (or end of data) */
+    }
+    return 0;
+}
+
+/* upload the file once, untouched, into buffers sized for K0 (marker list of list_cap entries, clean stream, tile status) */
+static int upload_file(struct gpujpeg_decoder* d, const uint8_t* image, size_t image_size, size_t ecs_begin, uint32_t list_cap, int stats)
+{
+    const size_t n_cta = (image_size - ecs_begin + 16) / 4096 + 2;
+    if ( grow_dev((void**)&d->d_file, &d->d_file_size, image_size + 64) ||
+         grow_dev((void**)&d->d_list_pos, &d->d_list_pos_size, (size_t)list_cap * 4) ||
+         grow_dev((void**)&d->d_list_code, &d->d_list_code_size, (size_t)list_cap) ||
+         grow_dev((void**)&d->d_list_cpos, &d->d_list_cpos_size, (size_t)list_cap * 4) ||
+         grow_dev((void**)&d->d_clean, &d->d_clean_size, image_size - ecs_begin + 64) ||
+         grow_mk_cta(d, n_cta * 8) ) {
+        GJ_ERR("Decoder device allocation failed: %s\n", gj_cuda_last_error());
+        return -1;
+    }
+    if ( stats && d->timers_ok ) gj_timer_start(&d->t_to, d->stream);
+    if ( gj_cuda_memcpy_h2d_async(d->d_file, image, image_size, d->stream) ) {
+        GJ_ERR("Decoder copy of compressed data failed: %s\n", gj_cuda_last_error());
+        return -1;
+    }
+    if ( stats && d->timers_ok ) gj_timer_stop(&d->t_to, d->stream);
+    return 0;
+}
+
+/* K4 (whole frame, or stripe by stripe with the copies to the host overlapped) straight into the buffer the caller asked for,
+ * the channel remap, the copy to the host; k3_part: the Huffman decoder runs per stripe as well (decode_striped) */
+static int k4_and_output(struct gpujpeg_decoder* d, struct gpujpeg_decoder_output* output, const struct gpujpeg_image_parameters* pi,
+                         const int comp_tq[GJ_MAX_COMP], int dequantize, int striped, const struct gj_huff_dec_args* k3_part, int stats)
+{
+    const struct gj_geometry* g = &d->geo;
+    const int to_host = output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER || output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_BUFFER;
+    uint8_t* d_out = d->d_raw;
+    if ( output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_CUDA_BUFFER ) {
+        if ( !output->data ) return -1;
+        d_out = output->data;
+    }
+    else if ( output->type == GPUJPEG_DECODER_OUTPUT_OPENGL_TEXTURE ) {
+        GJ_ERR("OpenGL texture output is not supported in this build.\n");
+        return -1;
+    }
+    uint8_t* h_dst = output->data;
+    if ( to_host ) {
+        if ( output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER ) {
+            if ( grow_host((void**)&d->h_raw, &d->h_raw_size, g->raw_size) ) return -1;
+            h_dst = d->h_raw;
+        }
+        else if ( !h_dst ) {
+            return -1;
+        }
+    }
+    int copied = 0;
+    if ( striped ) {
+        if ( decode_striped(d, comp_tq, d_out, h_dst, dequantize, k3_part) ) {
+            GJ_ERR("Inverse DCT / copy of raw data failed: %s\n", gj_cuda_last_error());
+            return -1;
+        }
+        copied = 1;
+    }
+    else if ( launch_k4(d, comp_tq, d_out, dequantize) ) {
+        GJ_ERR("Inverse DCT launch failed: %s\n", gj_cuda_last_error());
+        return -1;
+    }
+    if ( d->channel_remap ) {   /* on the finished raw image, in place [ref: src/gpujpeg_postprocessor.cu:450, 493] */
+        struct gj_raw_layout rl;
+        if ( gj_raw_layout_init(&rl, pi) ) return -1;
+        const int rc = gj_launch_channel_remap(d_out, &rl, pi->pixel_format, pi->width, pi->height, d->channel_remap, d->stream);
+        if ( rc == -2 ) GJ_ERR("Wrong channel remapping given, given %u channels but pixel format has %d!\n", d->channel_remap >> 24,
+                               gpujpeg_pixel_format_get_comp_count(pi->pixel_format));
+        else if ( rc == -3 ) GJ_ERR("Channel remapping is not implemented for chroma-subsampled pixel formats in this build.\n");
+        if ( rc ) return -1;
+    }
+    if ( stats && d->timers_ok ) {
+        gj_timer_stop(&d->t_dct, d->stream);
+        gj_timer_stop(&d->t_gpu, d->stream);
+    }
+
+    output->data_size = g->raw_size;
+    output->param_image = *pi;
+    if ( to_host ) {
+        if ( !copied ) {
+            if ( stats && d->timers_ok ) gj_timer_start(&d->t_from, d->stream);
+            if ( gj_cuda_memcpy_d2h_async(h_dst, d_out, g->raw_size, d->stream) ) {
+                GJ_ERR("Decoder copy of raw data failed: %s\n", gj_cuda_last_error());
+                return -1;
+            }
+            if ( stats && d->timers_ok ) gj_timer_stop(&d->t_from, d->stream);
+        }
+        output->data = h_dst;
+    }
+    else {
+        output->data = d_out;
+    }
+    return 0;
+}
+
+/* the per-stage timers of the frame just decoded (gpujpeg_decoder_get_stats) */
+static void record_stats(struct gpujpeg_decoder* d, const struct gpujpeg_decoder_output* output, const struct gpujpeg_image_parameters* pi,
+                         int stats, double t_reader_ms, double t_begin)
+{
+    d->stats_valid = 0;
+    if ( stats && d->timers_ok ) {
+        memset(&d->stats, 0, sizeof d->stats);
+        d->stats.duration_stream = t_reader_ms;
+        d->stats.duration_memory_to = gj_timer_ms(&d->t_to);
+        d->stats.duration_huffman_coder = gj_timer_ms(&d->t_huff);
+        d->stats.duration_dct_quantization = gj_timer_ms(&d->t_dct);
+        d->stats.duration_in_gpu = gj_timer_ms(&d->t_gpu);
+        if ( output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER || output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_BUFFER )
+            d->stats.duration_memory_from = gj_timer_ms(&d->t_from);
+        d->stats_valid = 1;
+        if ( d->verbose >= GPUJPEG_LL_STATUS ) {
+            fprintf(stderr, " -Stream Reader:     %10.3f ms\n", d->stats.duration_stream);
+            fprintf(stderr, " -Copy To Device:    %10.3f ms\n", d->stats.duration_memory_to);
+            fprintf(stderr, " -Huffman Decoder:   %10.3f ms\n", d->stats.duration_huffman_coder);
+            fprintf(stderr, " -DeQuant+IDCT+Post: %10.3f ms\n", d->stats.duration_dct_quantization);
+            fprintf(stderr, " -Copy From Device:  %10.3f ms\n", d->stats.duration_memory_from);
+            fprintf(stderr, "Decode Image GPU:    %10.3f ms (only in-GPU processing)\n", d->stats.duration_in_gpu);
+            fprintf(stderr, "Decode Image:        %10.3f ms\n", (gpujpeg_get_time() - t_begin) * 1000.0);
+            fprintf(stderr, "Decompressed Size:%13zu bytes %dx%d %s %s\n", output->data_size, pi->width, pi->height,
+                    gpujpeg_pixel_format_get_name(pi->pixel_format), gpujpeg_color_space_get_name(pi->color_space));
+        }
+    }
+}
+
+/* Progressive (SOF2) frames, from the first SOS on: the same upload, K0 and host marker walk as a baseline frame, then per
+ * scan the parameters and Huffman tables (those in force at its SOS), one table upload, the scan kernels in stream order
+ * (gj_progressive.cu) and the same K4 / output stage.  Segment-info tables and dec_opt_huffman / dec_opt_huffman_lanes do not
+ * apply; a restart marker with the wrong number is refused (no resynchronisation). */
+static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t image_size, struct gpujpeg_decoder_output* output,
+                              struct gj_stream* st, struct gpujpeg_parameters* p, struct gpujpeg_image_parameters* pi, size_t pos,
+                              int adobe, enum gpujpeg_color_space early_cs, int stats, double t_begin)
+{
+    static const int comp_tq[GJ_MAX_COMP] = {0, 1, 2, 3};   /* qinv_zz[c]: the table component c latched at its first scan */
+    d->last_valid = 0;
+    d->used_segment_info = 0;
+    if ( (!d->prog_scans && !(d->prog_scans = (struct gj_prog_scan*)malloc(sizeof(struct gj_prog_scan) * GJ_MAX_SCANS))) ||
+         (!d->h_prog_luts && !(d->h_prog_luts = (struct gj_dec_lut*)malloc(sizeof(struct gj_dec_lut) * GJ_MAX_SCANS * GJ_MAX_COMP))) ||
+         (!d->d_prog_luts && gj_cuda_malloc((void**)&d->d_prog_luts, sizeof(struct gj_dec_lut) * GJ_MAX_SCANS * GJ_MAX_COMP)) ) {
+        GJ_ERR("Decoder allocation failed: %s\n", gj_cuda_last_error());
+        return GPUJPEG_ERROR;
+    }
+    /* every restart marker of every scan goes into K0's list: at most one per two bytes of entropy-coded data */
+    const size_t ecs_begin = st->scan[0].begin;
+    const uint32_t list_cap = (uint32_t)((image_size - ecs_begin) / 2 + 1 + GJ_MK_OTHER_CAP);
+    uint32_t first_rank[GJ_MAX_SCANS], end_rank[GJ_MAX_SCANS], scan_cbegin[GJ_MAX_SCANS];
+    memset(first_rank, 0, sizeof first_rank);
+    memset(end_rank, 0, sizeof end_rank);
+    memset(scan_cbegin, 0, sizeof scan_cbegin);
+    if ( upload_file(d, image, image_size, ecs_begin, list_cap, stats) ||
+         k0_scan_extents(d, image, image_size, ecs_begin, list_cap, st, &pos, &adobe, first_rank, end_rank, scan_cbegin) ||
+         gj_reader_finish(st, adobe, d->verbose) )
+        return GPUJPEG_ERROR;
+    d->metadata = st->metadata;
+    if ( st->color_space != early_cs ) {
+        GJ_ERR("The stream's colour space (%s) is announced after its first scan header; not supported.\n",
+               gpujpeg_color_space_get_name(st->color_space));
+        return GPUJPEG_ERROR;
+    }
+    /* the coefficient planes are padded to whole MCUs as soon as any scan interleaves (libjpeg's DC scans do) */
+    int il = 0;
+    for ( int k = 0; k < st->scan_count; k++ )
+        il |= st->scan[k].ncomp > 1;
+    if ( il != p->interleaved ) {
+        p->interleaved = il;
+        if ( gpujpeg_decoder_init(d, p, pi) ) return GPUJPEG_ERROR;
+        if ( d->out_mode == GJ_OUT_GENERIC && grow_dev((void**)&d->d_planes, &d->d_planes_size, d->geo.coef_count) ) return GPUJPEG_ERROR;
+    }
+    const struct gj_geometry* g = &d->geo;
+
+    /* scans and their Huffman tables */
+    int nlut = 0;
+    for ( int k = 0; k < st->scan_count; k++ ) {
+        struct gj_prog_scan* S = &d->prog_scans[k];
+        if ( gj_prog_scan_init(g, st, k, st->restart_interval, S) ) {
+            GJ_ERR("Unsupported scan structure (progressive scan %d: components out of frame order or outside the frame).\n", k);
+            return GPUJPEG_ERROR;
+        }
+        S->first_rank = first_rank[k];
+        S->cbegin = scan_cbegin[k];
+        if ( end_rank[k] >= list_cap || end_rank[k] - first_rank[k] != (uint32_t)(S->seg_count - 1) ) {
+            GJ_ERR("JPEG stream has a broken restart-marker structure (progressive scan %d holds %u restart markers, expected %d)!\n",
+                   k, end_rank[k] - first_rank[k], S->seg_count - 1);
+            return GPUJPEG_ERROR;
+        }
+        S->lut0 = nlut;
+        const int nt = S->kind == GJ_PROG_DC_FIRST ? S->ncomp : S->kind == GJ_PROG_DC_REFINE ? 0 : 1;
+        for ( int i = 0; i < nt; i++ ) {
+            if ( !st->scan[k].huff_at[i] ) {
+                GJ_ERR("Huffman table used by progressive scan %d is missing!\n", k);
+                return GPUJPEG_ERROR;
+            }
+            struct gj_huff_spec spec;
+            gj_huff_spec_at(image, st->scan[k].huff_at[i], &spec);
+            if ( gj_dec_lut_build(&spec, &d->h_prog_luts[nlut++]) ) {
+                GJ_ERR("Invalid Huffman table (progressive scan %d)!\n", k);
+                return GPUJPEG_ERROR;
+            }
+        }
+    }
+    /* dequantisation by component: the table latched at the component's first scan */
+    memset(&d->h_tab, 0, sizeof d->h_tab);
+    for ( int c = 0; c < st->comp_count; c++ ) {
+        const uint8_t* q = st->have_comp_qt[c] ? st->comp_qt[c] : st->have_qt[st->comp_tq[c]] ? st->qt[st->comp_tq[c]] : NULL;
+        for ( int k = 0; q && k < 64; k++ )
+            d->h_tab.qinv_zz[c][k] = q[k];
+    }
+    const double t_reader_ms = (gpujpeg_get_time() - t_begin) * 1000.0;
+    if ( !d->tab_valid || memcmp(&d->h_tab, &d->h_tab_prev, sizeof d->h_tab) != 0 ) {
+        d->h_tab_prev = d->h_tab;
+        if ( gj_cuda_memcpy_h2d_async(d->d_tab, &d->h_tab_prev, sizeof d->h_tab, d->stream) ) return GPUJPEG_ERROR;
+        d->tab_valid = 1;
+    }
+    if ( nlut && gj_cuda_memcpy_h2d_async(d->d_prog_luts, d->h_prog_luts, sizeof(struct gj_dec_lut) * (size_t)nlut, d->stream) )
+        return GPUJPEG_ERROR;
+
+    struct gj_prog_args* a = &d->last_prog;
+    memset(a, 0, sizeof *a);
+    a->scans = d->prog_scans;
+    a->scan_count = st->scan_count;
+    a->d_luts = d->d_prog_luts;
+    a->d_clean = (const uint32_t*)d->d_clean;
+    a->d_list_cpos = d->d_list_cpos;
+    a->d_list_code = d->d_list_code;
+    a->d_error = d->d_mk + 3;
+    a->d_coef = d->d_coef;
+    a->coef_count = g->coef_count;
+    a->dequantize = d->idct_flavour == 0;
+    a->comp_count = g->comp_count;
+    for ( int c = 0; c < g->comp_count; c++ )
+        a->comp_blk_off[c] = g->comp[c].blk_off;
+    a->d_tables = d->d_tab;
+    d->last_args.file_size = image_size;   /* what a resident re-run of K0 needs */
+    d->last_ecs_begin = ecs_begin;
+    d->last_list_cap = list_cap;
+    d->last_progressive = 1;
+    d->last_valid = 1;
+    if ( stats && d->timers_ok ) {
+        gj_timer_start(&d->t_gpu, d->stream);
+        gj_timer_start(&d->t_huff, d->stream);
+    }
+    if ( gj_launch_progressive_decode(a, d->stream) ) {
+        GJ_ERR("Progressive Huffman decoder launch failed: %s\n", gj_cuda_last_error());
+        return GPUJPEG_ERROR;
+    }
+    if ( stats && d->timers_ok ) {
+        gj_timer_stop(&d->t_huff, d->stream);
+        gj_timer_start(&d->t_dct, d->stream);
+    }
+    const int to_host = output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER || output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_BUFFER;
+    const int striped = to_host && !stats && stripes_usable(d);
+    if ( k4_and_output(d, output, pi, comp_tq, a->dequantize, striped, NULL, stats) ) return GPUJPEG_ERROR;
+    if ( gj_cuda_memcpy_d2h_async(d->h_mk, d->d_mk, 16, d->stream) || gj_cuda_stream_sync(d->stream) ) {
+        GJ_ERR("Decoder failed: %s\n", gj_cuda_last_error());
+        return GPUJPEG_ERROR;
+    }
+    if ( d->h_mk[3] ) {
+        GJ_ERR("Restart marker with the wrong number in a progressive scan; not supported.\n");
+        d->last_valid = 0;
+        return GPUJPEG_ERROR;
+    }
+    output->metadata = &d->metadata;
+    record_stats(d, output, pi, stats, t_reader_ms, t_begin);
+    return GPUJPEG_NOERR;
+}
+
 /* [ref: src/gpujpeg_decoder.c:234-469] */
 int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t image_size,
                            struct gpujpeg_decoder_output* output)
@@ -665,7 +1018,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         }
     }
     st.interleaved = st.scan[0].ncomp > 1;
-    if ( st.interleaved && st.scan[0].ncomp != st.comp_count ) {
+    if ( !st.progressive && st.interleaved && st.scan[0].ncomp != st.comp_count ) {
         GJ_ERR("Unsupported scan structure (%d components in first scan).\n", st.scan[0].ncomp);
         return GPUJPEG_ERROR;
     }
@@ -714,25 +1067,12 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     if ( out_mode == GJ_OUT_GENERIC && grow_dev((void**)&d->d_planes, &d->d_planes_size, d->geo.coef_count) ) return GPUJPEG_ERROR;
     const struct gj_geometry* g = &d->geo;
 
+    if ( st.progressive ) return decode_progressive(d, image, image_size, output, &st, &p, &pi, pos, adobe, early_cs, stats, t_begin);
+
     /* ---- upload the file once, untouched; K0 builds the marker list on the device ---- */
     const size_t ecs_begin = st.scan[0].begin;
     const uint32_t list_cap = (uint32_t)g->seg_count + GJ_MK_OTHER_CAP;
-    const size_t n_cta = (image_size - ecs_begin + 16) / 4096 + 2;
-    if ( grow_dev((void**)&d->d_file, &d->d_file_size, image_size + 64) ||
-         grow_dev((void**)&d->d_list_pos, &d->d_list_pos_size, (size_t)list_cap * 4) ||
-         grow_dev((void**)&d->d_list_code, &d->d_list_code_size, (size_t)list_cap) ||
-         grow_dev((void**)&d->d_list_cpos, &d->d_list_cpos_size, (size_t)list_cap * 4) ||
-         grow_dev((void**)&d->d_clean, &d->d_clean_size, image_size - ecs_begin + 64) ||
-         grow_mk_cta(d, n_cta * 8) ) {
-        GJ_ERR("Decoder device allocation failed: %s\n", gj_cuda_last_error());
-        return GPUJPEG_ERROR;
-    }
-    if ( stats && d->timers_ok ) gj_timer_start(&d->t_to, d->stream);
-    if ( gj_cuda_memcpy_h2d_async(d->d_file, image, image_size, d->stream) ) {
-        GJ_ERR("Decoder copy of compressed data failed: %s\n", gj_cuda_last_error());
-        return GPUJPEG_ERROR;
-    }
-    if ( stats && d->timers_ok ) gj_timer_stop(&d->t_to, d->stream);
+    if ( upload_file(d, image, image_size, ecs_begin, list_cap, stats) ) return GPUJPEG_ERROR;
     uint32_t first_rank[GJ_MAX_COMP] = {0, 0, 0, 0}, end_rank[GJ_MAX_COMP] = {0, 0, 0, 0}, scan_cbegin[GJ_MAX_COMP] = {0, 0, 0, 0};
     /* ---- scans split by the stream's own segment-info tables (no K0, no round trip), or ... ---- */
     const int by_table = split_by_segment_info(d, image, image_size, &st, &pos, &adobe);
@@ -746,74 +1086,8 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     }
     else {
     /* ---- ... K0 builds the marker list and the clean stream on the device ---- */
-    /* d_mk: [0] total markers, [1] non-RST markers, [2] list overflow, [3] restart sequence error (K3), [5] clean bytes,
-     *       [8..] {rank, position, code, clean position} of the non-RST markers */
-    if ( gj_launch_marker_scan(d->d_file, ecs_begin, image_size, d->d_cta, d->d_list_pos, d->d_list_code, d->d_list_cpos,
-                               list_cap, d->d_clean, d->d_mk, d->d_mk + 8, GJ_MK_OTHER_CAP, d->stream) ||
-         gj_cuda_memcpy_d2h_async(d->h_mk, d->d_mk, GJ_MK_WORDS * 4, d->stream) ||
-         gj_cuda_stream_sync(d->stream) ) {
-        GJ_ERR("Marker scan failed: %s\n", gj_cuda_last_error());
+    if ( k0_scan_extents(d, image, image_size, ecs_begin, list_cap, &st, &pos, &adobe, first_rank, end_rank, scan_cbegin) )
         return GPUJPEG_ERROR;
-    }
-
-    /* ---- host reader, part 2: scan extents from the marker list, marker segments between scans by length ---- */
-    const uint32_t n_other = d->h_mk[1];
-    if ( n_other == 0 || n_other > GJ_MK_OTHER_CAP ) {
-        GJ_ERR("JPEG stream has %u restart markers / %u other markers in its scan data, expected %d restart segments "
-               "for a %dx%d image with restart interval %d!\n", d->h_mk[0], n_other, g->seg_count, st.width, st.height,
-               st.restart_interval);
-        return GPUJPEG_ERROR;
-    }
-    uint32_t* other = d->h_mk + 8; /* insertion sort by position: a handful of entries */
-    for ( uint32_t i = 1; i < n_other; i++ ) {
-        uint32_t t[4] = {other[4 * i], other[4 * i + 1], other[4 * i + 2], other[4 * i + 3]};
-        uint32_t j = i;
-        while ( j > 0 && other[4 * (j - 1) + 1] > t[1] ) {
-            memcpy(other + 4 * j, other + 4 * (j - 1), 16);
-            j--;
-        }
-        memcpy(other + 4 * j, t, 16);
-    }
-    /* per scan, from the marker report alone (no second kernel, no walk over the entropy-coded bytes): where it ends,
-     * how many markers lie in front of it, how many restart markers it holds, where its clean bytes start */
-    for ( int k = 0; k < st.scan_count; k++ ) {
-        /* a scan ends at the first marker that is not RSTn: inside entropy-coded data that test is exact */
-        size_t e1 = 0;
-        int last_before = -1;
-        for ( uint32_t i = 0; i < n_other; i++ ) {
-            if ( other[4 * i + 1] >= st.scan[k].begin ) {
-                e1 = other[4 * i + 1];
-                end_rank[k] = other[4 * i];
-                break;
-            }
-            last_before = (int)i;
-        }
-        if ( last_before >= 0 ) {
-            /* the last marker in front of the scan (its SOS): everything up to the scan's first byte that K0 kept
-             * belongs to the clean stream too -- the same keep rule, applied to the few header bytes */
-            const uint32_t* m = other + 4 * last_before;
-            first_rank[k] = m[0] + 1;
-            uint32_t c = m[3];
-            if ( st.scan[k].begin - m[1] > 4096 ) {
-                GJ_ERR("Unsupported scan structure (no marker in front of scan %d).\n", k);
-                return GPUJPEG_ERROR;
-            }
-            for ( size_t q = (size_t)m[1] + 2; q < st.scan[k].begin; q++ ) {
-                const int b0 = image[q], b1 = q + 1 < image_size ? image[q + 1] : 0, prev = image[q - 1];
-                if ( !((b0 == 0xFF && b1 != 0) || (prev == 0xFF && b0 != 0xFF)) ) c++;
-            }
-            scan_cbegin[k] = c;
-        }
-        if ( e1 == 0 ) {
-            GJ_ERR("JPEG data unexpected ended while reading SOS marker!\n");
-            return GPUJPEG_ERROR;
-        }
-        st.scan[k].end = e1;
-        pos = e1;
-        const int r = gj_reader_walk(image, image_size, &pos, &st, &adobe);
-        if ( r < 0 ) return GPUJPEG_ERROR;
-        if ( r == 0 ) break; /* EOI (or end of data) */
-    }
     }   /* K0 path */
     if ( gj_reader_finish(&st, adobe, d->verbose) ) return GPUJPEG_ERROR;
     d->metadata = st.metadata;   /* handed out with the output [ref: src/gpujpeg_reader.c:1626-1636, src/gpujpeg_decoder.c:466] */
@@ -956,6 +1230,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     d->last_list_cap = list_cap;
     memcpy(d->last_tq, st.comp_tq, sizeof d->last_tq);
     d->last_valid = 1;
+    d->last_progressive = 0;
   for ( int pass = 0;; pass++ ) {
     if ( resync ) {
         if ( resync_segments(d, &st, first_rank, end_rank, scan_cbegin, &ha) ) return GPUJPEG_ERROR;
@@ -979,68 +1254,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         gj_timer_start(&d->t_dct, d->stream);
     }
 
-    /* ---- K4, straight into the buffer the caller asked for ---- */
-    uint8_t* d_out = d->d_raw;
-    if ( output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_CUDA_BUFFER ) {
-        if ( !output->data ) return GPUJPEG_ERROR;
-        d_out = output->data;
-    }
-    else if ( output->type == GPUJPEG_DECODER_OUTPUT_OPENGL_TEXTURE ) {
-        GJ_ERR("OpenGL texture output is not supported in this build.\n");
-        return GPUJPEG_ERROR;
-    }
-    uint8_t* h_dst = output->data;
-    if ( to_host ) {
-        if ( output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER ) {
-            if ( grow_host((void**)&d->h_raw, &d->h_raw_size, g->raw_size) ) return GPUJPEG_ERROR;
-            h_dst = d->h_raw;
-        }
-        else if ( !h_dst ) {
-            return GPUJPEG_ERROR;
-        }
-    }
-    int copied = 0;
-    if ( striped ) {
-        if ( decode_striped(d, st.comp_tq, d_out, h_dst, ha.dequantize, k3_striped ? &ha : NULL) ) {
-            GJ_ERR("Inverse DCT / copy of raw data failed: %s\n", gj_cuda_last_error());
-            return GPUJPEG_ERROR;
-        }
-        copied = 1;
-    }
-    else if ( launch_k4(d, st.comp_tq, d_out, ha.dequantize) ) {
-        GJ_ERR("Inverse DCT launch failed: %s\n", gj_cuda_last_error());
-        return GPUJPEG_ERROR;
-    }
-    if ( d->channel_remap ) {   /* on the finished raw image, in place [ref: src/gpujpeg_postprocessor.cu:450, 493] */
-        struct gj_raw_layout rl;
-        if ( gj_raw_layout_init(&rl, &pi) ) return GPUJPEG_ERROR;
-        const int rc = gj_launch_channel_remap(d_out, &rl, pi.pixel_format, pi.width, pi.height, d->channel_remap, d->stream);
-        if ( rc == -2 ) GJ_ERR("Wrong channel remapping given, given %u channels but pixel format has %d!\n", d->channel_remap >> 24,
-                               gpujpeg_pixel_format_get_comp_count(pi.pixel_format));
-        else if ( rc == -3 ) GJ_ERR("Channel remapping is not implemented for chroma-subsampled pixel formats in this build.\n");
-        if ( rc ) return GPUJPEG_ERROR;
-    }
-    if ( stats && d->timers_ok ) {
-        gj_timer_stop(&d->t_dct, d->stream);
-        gj_timer_stop(&d->t_gpu, d->stream);
-    }
-
-    output->data_size = g->raw_size;
-    output->param_image = pi;
-    if ( to_host ) {
-        if ( !copied ) {
-            if ( stats && d->timers_ok ) gj_timer_start(&d->t_from, d->stream);
-            if ( gj_cuda_memcpy_d2h_async(h_dst, d_out, g->raw_size, d->stream) ) {
-                GJ_ERR("Decoder copy of raw data failed: %s\n", gj_cuda_last_error());
-                return GPUJPEG_ERROR;
-            }
-            if ( stats && d->timers_ok ) gj_timer_stop(&d->t_from, d->stream);
-        }
-        output->data = h_dst;
-    }
-    else {
-        output->data = d_out;
-    }
+    if ( k4_and_output(d, output, &pi, st.comp_tq, ha.dequantize, striped, k3_striped ? &ha : NULL, stats) ) return GPUJPEG_ERROR;
     if ( gj_cuda_memcpy_d2h_async(d->h_mk, d->d_mk, 16, d->stream) || gj_cuda_stream_sync(d->stream) ) {
         GJ_ERR("Decoder failed: %s\n", gj_cuda_last_error());
         return GPUJPEG_ERROR;
@@ -1062,29 +1276,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
   }
     output->metadata = &d->metadata;
 
-    d->stats_valid = 0;
-    if ( stats && d->timers_ok ) {
-        memset(&d->stats, 0, sizeof d->stats);
-        d->stats.duration_stream = t_reader_ms;
-        d->stats.duration_memory_to = gj_timer_ms(&d->t_to);
-        d->stats.duration_huffman_coder = gj_timer_ms(&d->t_huff);
-        d->stats.duration_dct_quantization = gj_timer_ms(&d->t_dct);
-        d->stats.duration_in_gpu = gj_timer_ms(&d->t_gpu);
-        if ( output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER || output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_BUFFER )
-            d->stats.duration_memory_from = gj_timer_ms(&d->t_from);
-        d->stats_valid = 1;
-        if ( d->verbose >= GPUJPEG_LL_STATUS ) {
-            fprintf(stderr, " -Stream Reader:     %10.3f ms\n", d->stats.duration_stream);
-            fprintf(stderr, " -Copy To Device:    %10.3f ms\n", d->stats.duration_memory_to);
-            fprintf(stderr, " -Huffman Decoder:   %10.3f ms\n", d->stats.duration_huffman_coder);
-            fprintf(stderr, " -DeQuant+IDCT+Post: %10.3f ms\n", d->stats.duration_dct_quantization);
-            fprintf(stderr, " -Copy From Device:  %10.3f ms\n", d->stats.duration_memory_from);
-            fprintf(stderr, "Decode Image GPU:    %10.3f ms (only in-GPU processing)\n", d->stats.duration_in_gpu);
-            fprintf(stderr, "Decode Image:        %10.3f ms\n", (gpujpeg_get_time() - t_begin) * 1000.0);
-            fprintf(stderr, "Decompressed Size:%13zu bytes %dx%d %s %s\n", output->data_size, pi.width, pi.height,
-                    gpujpeg_pixel_format_get_name(pi.pixel_format), gpujpeg_color_space_get_name(pi.color_space));
-        }
-    }
+    record_stats(d, output, &pi, stats, t_reader_ms, t_begin);
     return GPUJPEG_NOERR;
 }
 
@@ -1237,6 +1429,17 @@ GPUJPEG_API int gpujpegx_decoder_used_segment_info(const struct gpujpeg_decoder*
 GPUJPEG_API int gpujpegx_decoder_run_resident(struct gpujpeg_decoder* d, uint8_t* d_out, int stage_mask)
 {
     if ( !d || !d->last_valid ) return -1;
+    if ( d->last_progressive ) {
+        /* bit 2 K0, bit 0 the zeroing, every scan and the dequantisation, bit 1 K4 */
+        static const int comp_tq[GJ_MAX_COMP] = {0, 1, 2, 3};
+        if ( (stage_mask & 4) &&
+             gj_launch_marker_scan(d->d_file, d->last_ecs_begin, d->last_args.file_size, d->d_cta, d->d_list_pos, d->d_list_code,
+                                   d->d_list_cpos, d->last_list_cap, d->d_clean, d->d_mk, d->d_mk + 8, GJ_MK_OTHER_CAP, d->stream) )
+            return -1;
+        if ( (stage_mask & 1) && gj_launch_progressive_decode(&d->last_prog, d->stream) ) return -1;
+        if ( (stage_mask & 2) && launch_k4(d, comp_tq, d_out ? d_out : d->d_raw, d->last_prog.dequantize) ) return -1;
+        return 0;
+    }
     if ( (stage_mask & 4) && !d->used_segment_info &&
          gj_launch_marker_scan(d->d_file, d->last_ecs_begin, d->last_args.file_size, d->d_cta, d->d_list_pos, d->d_list_code,
                                d->d_list_cpos, d->last_list_cap, d->d_clean, d->d_mk, d->d_mk + 8, GJ_MK_OTHER_CAP, d->stream) )
@@ -1253,5 +1456,5 @@ GPUJPEG_API int gpujpegx_decoder_get_coefficients(struct gpujpeg_decoder* d, int
 {
     if ( !d || !d->initialised || !d->last_valid || count != d->geo.coef_count ) return -1;
     if ( gj_coef_to_host_natural(d->d_coef, count, out, d->stream) ) return -1;
-    return d->last_args.dequantize ? 1 : 0;
+    return (d->last_progressive ? d->last_prog.dequantize : d->last_args.dequantize) ? 1 : 0;
 }

@@ -16,6 +16,8 @@
 #include <stdint.h>
 #include <math.h>
 
+#include "gj_internal.h"
+
 #if defined(__CUDA_ARCH__)
 #define GJ_HD __host__ __device__ __forceinline__
 #define GJ_FADD(a, b) __fadd_rn((a), (b))
@@ -405,5 +407,219 @@ GJ_HD int gj_category(int v)
 GJ_HD unsigned gj_value_bits(int v, int size) { return (unsigned)(v < 0 ? v - 1 : v) & ((1u << size) - 1u); }
 /* inverse [ref: src/gpujpeg_huffman_cpu_decoder.c:169-204] */
 GJ_HD int gj_extend(int bits, int size) { return bits < (1 << (size - 1)) ? bits - (1 << size) + 1 : bits; }
+
+/* ------------------------------------------------------------------------------------------- */
+/* progressive Huffman decoding (T.81 G.2), one restart segment per thread: k_prog_decode         */
+
+/* Bits of one restart segment of K0's clean stream (big-endian 32-bit words, stuffing and markers removed): a 64-bit
+ * buffer, left-aligned, refilled a word at a time from a one-word lookahead.  Bits past the segment's end read as zeros
+ * (as in libjpeg) and no word behind the segment's last one is ever loaded. */
+struct gj_prog_bits {
+    const uint32_t* wp;   /* the word behind `nxt` */
+    uint64_t acc;         /* the next n bits of the segment, from bit 63 down */
+    int n;
+    uint32_t nxt;         /* lookahead word */
+    uint32_t left;        /* segment bits from nxt's first bit on */
+};
+GJ_HD uint32_t gj_prog_ld(const uint32_t* p)
+{
+#if defined(__CUDA_ARCH__)
+    return __ldg(p);
+#else
+    return *p;
+#endif
+}
+GJ_HD uint32_t gj_prog_word(gj_prog_bits& r)
+{
+    uint32_t v = r.nxt;
+    if ( r.left < 32u ) {
+        v = r.left ? v & (0xFFFFFFFFu << (32u - r.left)) : 0u;
+        r.left = 0;
+    }
+    else {
+        r.left -= 32u;
+    }
+    r.nxt = r.left ? gj_prog_ld(r.wp) : 0u;
+    if ( r.left ) r.wp++;
+    return v;
+}
+GJ_HD void gj_prog_fill(gj_prog_bits& r)
+{
+    while ( r.n <= 32 ) {
+        r.acc |= (uint64_t)gj_prog_word(r) << (32 - r.n);
+        r.n += 32;
+    }
+}
+/* the segment = clean bytes [cs, ce) */
+GJ_HD void gj_prog_bits_init(gj_prog_bits& r, const uint32_t* clean, uint32_t cs, uint32_t ce)
+{
+    const uint32_t skip = (cs & 3u) * 8u;
+    r.left = ce > cs ? (ce - cs) * 8u + skip : 0u;
+    r.acc = 0;
+    r.n = 0;
+    r.wp = clean + (cs >> 2);
+    r.nxt = r.left ? gj_prog_ld(r.wp) : 0u;
+    if ( r.left ) r.wp++;
+    gj_prog_fill(r);
+    r.acc <<= skip;
+    r.n -= (int)skip;
+}
+/* `len` (0..16) bits as an unsigned number */
+GJ_HD int gj_prog_get(gj_prog_bits& r, int len)
+{
+    if ( len == 0 ) return 0;
+    gj_prog_fill(r);
+    const int v = (int)(r.acc >> (64 - len));
+    r.acc <<= len;
+    r.n -= len;
+    return v;
+}
+/* one Huffman symbol: 9-bit lookup, then the canonical search of gj_dec_lut; a code no table entry covers consumes 16
+ * bits and reads as symbol 0 (end of band / DC size 0), as the baseline decoders treat garbage */
+GJ_HD int gj_prog_symbol(gj_prog_bits& r, const gj_dec_lut& t)
+{
+    gj_prog_fill(r);
+    const uint32_t peek = (uint32_t)(r.acc >> 48);
+    const uint32_t e = t.look[peek >> (16 - GJ_DEC_LOOK_BITS)];
+    int l = (int)(e & 15u);
+    int sym = (int)(e >> 4);
+    if ( !l ) {
+        l = GJ_DEC_LOOK_BITS + 1;
+        while ( l <= 16 && peek >= t.maxcode[l] ) l++;
+        if ( l > 16 ) {
+            l = 16;
+            sym = 0;
+        }
+        else {
+            sym = t.vals[((int)(peek >> (16 - l)) + t.valoff[l]) & 255];
+        }
+    }
+    r.acc <<= l;
+    r.n -= l;
+    return sym;
+}
+
+/* what a segment carries from block to block: DC predictors and the remaining end-of-band run */
+struct gj_prog_state {
+    int pred[GJ_MAX_COMP];
+    int eobrun;
+};
+
+/* G.2.1 / G.1.2.1: DC of the first scan: a difference of the point-transformed DC, stored as value << Al */
+GJ_HD void gj_prog_dc_first(gj_prog_bits& r, const gj_dec_lut& t, int& pred, int al, int16_t* blk)
+{
+    const int s = gj_prog_symbol(r, t) & 15;
+    const int diff = s ? gj_extend(gj_prog_get(r, s), s) : 0;
+    pred = (int16_t)(pred + diff);   /* (only the low 16 bits are ever stored: corrupt data cannot overflow) */
+    blk[0] = (int16_t)((unsigned)pred << al);
+}
+/* G.1.2.1: one more bit of the DC, bit position Al */
+GJ_HD void gj_prog_dc_refine(gj_prog_bits& r, int al, int16_t* blk)
+{
+    if ( gj_prog_get(r, 1) ) blk[0] = (int16_t)(blk[0] | (1 << al));
+}
+/* G.1.2.2: AC band [ss, se] of a first scan; EOBn symbols start a run of blocks whose band is all zero */
+GJ_HD void gj_prog_ac_first(gj_prog_bits& r, const gj_dec_lut& t, int& eobrun, int ss, int se, int al, int16_t* blk)
+{
+    if ( eobrun > 0 ) {
+        eobrun--;
+        return;
+    }
+    for ( int k = ss; k <= se; ) {
+        const int rs = gj_prog_symbol(r, t);
+        const int run = rs >> 4, s = rs & 15;
+        if ( s ) {
+            k += run;
+            const int v = gj_extend(gj_prog_get(r, s), s);
+            if ( k <= se ) blk[k] = (int16_t)(v * (1 << al));
+            k++;
+        }
+        else if ( run == 15 ) {
+            k += 16;   /* ZRL */
+        }
+        else {
+            eobrun = (1 << run) - 1 + gj_prog_get(r, run);   /* EOBn: this block and (1 << run) - 1 + bits more */
+            break;
+        }
+    }
+}
+/* G.1.2.3: one more bit of AC band [ss, se] at position Al.  Coefficients that are non-zero already get a correction bit
+ * each; a coefficient that becomes non-zero is coded as run (of zero-history coefficients to skip) / size 1 + sign */
+GJ_HD void gj_prog_ac_refine(gj_prog_bits& r, const gj_dec_lut& t, int& eobrun, int ss, int se, int al, int16_t* blk)
+{
+    const int p1 = 1 << al;
+    int k = ss;
+    auto correct = [&](int kk) {   /* correction bit of a coefficient with history */
+        const int c = blk[kk];
+        if ( gj_prog_get(r, 1) && (c & p1) == 0 ) blk[kk] = (int16_t)(c >= 0 ? c + p1 : c - p1);
+    };
+    if ( eobrun == 0 ) {
+        for ( ; k <= se; k++ ) {
+            const int rs = gj_prog_symbol(r, t);
+            int run = rs >> 4;
+            const int s = rs & 15;
+            int v = 0;
+            if ( s ) {
+                v = gj_prog_get(r, 1) ? p1 : -p1;   /* (a size other than 1 is invalid here: read as 1) */
+            }
+            else if ( run != 15 ) {
+                eobrun = (1 << run) + gj_prog_get(r, run);   /* EOBn, this block included */
+                break;
+            }
+            /* skip `run` zero-history coefficients (ZRL: 16), correcting the ones with history on the way */
+            for ( ; k <= se; k++ ) {
+                if ( blk[k] != 0 ) correct(k);
+                else if ( run-- == 0 ) break;
+            }
+            if ( v && k <= se ) blk[k] = (int16_t)v;
+        }
+    }
+    if ( eobrun > 0 ) {
+        for ( ; k <= se; k++ )
+            if ( blk[k] != 0 ) correct(k);
+        eobrun--;
+    }
+}
+
+/* Block i of unit (MCU) u of a scan -> its index in the coefficient buffer, clamped to the component's plane (the host
+ * checks that a scan fits its planes, gj_prog_scan_init; the clamp only keeps an inconsistent scan inside the buffer) */
+GJ_HD long gj_prog_block(const gj_prog_scan& S, int u, int i, int& ci)
+{
+    ci = S.ncomp == 1 ? 0 : S.idx_ci[i];
+    const int my = u / S.units_x, mx = u - my * S.units_x;
+    long b = S.ncomp == 1 ? (long)my * S.bcx[0] + mx   /* one block per unit, the component's own block grid */
+                          : (long)(my * S.vs[ci] + S.idx_dy[i]) * S.bcx[ci] + mx * S.hs[ci] + S.idx_dx[i];
+    b = b < 0 ? 0 : b >= S.nblk[ci] ? S.nblk[ci] - 1 : b;
+    return S.blk_off[ci] + b;
+}
+
+/* Restart segment `seg` of a scan, clean bytes [cs, ce): every block of its units in coding order.  KIND is the scan's
+ * GJ_PROG_* kind; `tab` the scan's tables by scan component (unused by DC refinements).  Predictors and the end-of-band
+ * run start at zero, as after every restart marker.  Values go into the zig-zag coefficient buffer, raw (not dequantised),
+ * and only inside the scan's band and the component's plane. */
+template <int KIND>
+GJ_HD void gj_prog_segment(const gj_prog_scan& S, const gj_dec_lut* tab, const uint32_t* clean, uint32_t cs, uint32_t ce, int seg,
+                           int16_t* coef)
+{
+    gj_prog_bits r;
+    gj_prog_bits_init(r, clean, cs, ce);
+    gj_prog_state st;
+    for ( int c = 0; c < GJ_MAX_COMP; c++ )
+        st.pred[c] = 0;
+    st.eobrun = 0;
+    const int u0 = seg * S.seg_units;
+    const int u1 = u0 + S.seg_units < S.units ? u0 + S.seg_units : S.units;
+    const int ss = S.ss < 1 ? (KIND >= GJ_PROG_AC_FIRST ? 1 : 0) : S.ss > 63 ? 63 : S.ss;
+    const int se = S.se > 63 ? 63 : S.se;
+    for ( int u = u0; u < u1; u++ )
+        for ( int i = 0; i < S.bpm; i++ ) {
+            int ci;
+            int16_t* blk = coef + gj_prog_block(S, u, i, ci) * 64;
+            if ( KIND == GJ_PROG_DC_FIRST ) gj_prog_dc_first(r, tab[ci], st.pred[ci], S.al, blk);
+            else if ( KIND == GJ_PROG_DC_REFINE ) gj_prog_dc_refine(r, S.al, blk);
+            else if ( KIND == GJ_PROG_AC_FIRST ) gj_prog_ac_first(r, tab[0], st.eobrun, ss, se, S.al, blk);
+            else gj_prog_ac_refine(r, tab[0], st.eobrun, ss, se, S.al, blk);
+        }
+}
 
 #endif /* GJ_DEVICE_CUH */

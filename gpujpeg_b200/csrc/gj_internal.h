@@ -204,13 +204,22 @@ size_t gj_write_segment_info_headers(uint8_t* out, int scan_index, int segment_c
 size_t gj_segment_info_entry_offset(int index);
 
 /* ---- codestream reader (gj_reader.c)  [ref: src/gpujpeg_reader.c] ---- */
+/* Scans a progressive (SOF2) frame may have: libjpeg's scripts use 6-10, hand-written ones rarely more than about 20.  A
+ * baseline frame keeps its limit of GJ_MAX_COMP scans. */
+#define GJ_MAX_SCANS 64
 struct gj_scan_info {
     int ncomp;
     int comp[GJ_MAX_COMP];
     int td[GJ_MAX_COMP], ta[GJ_MAX_COMP];
+    int ss, se, ah, al;   /* spectral selection and successive approximation (T.81 B.2.3); baseline: 0, 63, 0, 0 */
+    /* progressive frames: file offset of the DHT entry (its Tc/Th byte) in force at the SOS for the table component k of
+     * the scan uses -- DC for a DC-first scan, AC for an AC scan --, 0 = no such table was defined (a DC refinement uses none) */
+    size_t huff_at[GJ_MAX_COMP];
     size_t begin, end; /* entropy-coded bytes [begin,end) in the file */
     int first_segment, segment_count;
 };
+/* the table a DHT entry at file offset `at` (as recorded in gj_scan_info.huff_at) defines; the walk has checked it */
+void gj_huff_spec_at(const uint8_t* data, size_t at, struct gj_huff_spec* spec);
 /* APP13 "segment info" headers met in front of a scan [ref: src/gpujpeg_reader.c:229-249]: pieces of one table of
  * big-endian 32-bit positions (every restart segment's first byte relative to the scan's first byte, then the scan's end) */
 #define GJ_SEGINFO_MAX_PIECES 64
@@ -228,9 +237,17 @@ struct gj_stream {
     int have_qt[4];
     struct gj_huff_spec huff[2][4]; /* [class][id] */
     int have_huff[2][4];
+    size_t huff_at[2][4];           /* file offset of the DHT entry that defined [class][id] */
+    int progressive;                /* SOF2: Huffman-coded progressive DCT (T.81 Annex G) */
+    /* progressive frames: per component and zig-zag coefficient, 1 + the Al of the last scan that coded it (0 = none yet),
+     * as T.81 G.1.1.1.2 requires every refinement to continue; and the quantisation table latched at the component's first
+     * scan (have_comp_qt) */
+    uint8_t coef_bits[GJ_MAX_COMP][64];
+    uint8_t comp_qt[GJ_MAX_COMP][64];
+    int have_comp_qt[GJ_MAX_COMP];
     int scan_count;
-    struct gj_scan_info scan[GJ_MAX_COMP];
-    struct gj_seginfo seginfo[GJ_MAX_COMP];   /* [scan]: the table in front of the scan's SOS, if any */
+    struct gj_scan_info scan[GJ_MAX_SCANS];
+    struct gj_seginfo seginfo[GJ_MAX_COMP];   /* [scan]: the table in front of the scan's SOS, if any (baseline scans only) */
     struct gj_seginfo seginfo_pending;        /* headers met since the last SOS */
     enum gpujpeg_color_space color_space;
     int spiff_color_space;   /* colour space named by a SPIFF header, GPUJPEG_NONE (0) if there is none */
@@ -386,6 +403,45 @@ struct gj_huff_dec_args {
 };
 int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_stream_t stream);
 int gj_huffman_decode_parts_eligible(const struct gj_huff_dec_args* a);   /* part_seg_lo / part_seg_hi may be used */
+
+/* Progressive frames (gj_progressive.cu): one scan of a SOF2 frame as k_prog_decode sees it.  An interleaved scan (DC
+ * only) codes MCUs of the frame's MCU grid; a non-interleaved one codes the component's own ceil(w_c/8) x ceil(h_c/8)
+ * blocks -- one block per MCU, so that the restart interval counts blocks -- inside its (possibly MCU-padded) plane. */
+enum { GJ_PROG_DC_FIRST = 0, GJ_PROG_DC_REFINE = 1, GJ_PROG_AC_FIRST = 2, GJ_PROG_AC_REFINE = 3 };
+struct gj_prog_scan {
+    int kind;                      /* GJ_PROG_* */
+    int ss, se, ah, al;
+    int ncomp;                     /* components in the scan */
+    int bpm;                       /* blocks per MCU */
+    int units, units_x;            /* MCUs of the scan, MCUs per row */
+    int seg_units;                 /* MCUs per restart segment */
+    int seg_count;
+    int lut0;                      /* component i of the scan decodes with table lut0 + i of the frame's table array */
+    uint32_t first_rank, cbegin;   /* K0: markers in front of the scan, clean-stream position of its first byte */
+    int blk_off[GJ_MAX_COMP], bcx[GJ_MAX_COMP], nblk[GJ_MAX_COMP], hs[GJ_MAX_COMP], vs[GJ_MAX_COMP];   /* by scan component */
+    uint8_t idx_ci[GJ_MAX_MCU_BLOCKS], idx_dx[GJ_MAX_MCU_BLOCKS], idx_dy[GJ_MAX_MCU_BLOCKS];          /* block i of an MCU */
+};
+/* scan k of a progressive stream on the frame geometry g (which must be the interleaved one if any scan interleaves);
+ * 0 on success, -1 if the scan does not fit the geometry */
+int gj_prog_scan_init(const struct gj_geometry* g, const struct gj_stream* s, int k, int restart_interval, struct gj_prog_scan* out);
+
+struct gj_prog_args {
+    const struct gj_prog_scan* scans;   /* host array, scan_count entries */
+    int scan_count;
+    const struct gj_dec_lut* d_luts;    /* every scan's Huffman tables, one copy per frame */
+    const uint32_t* d_clean;            /* K0's clean stream and marker list */
+    const uint32_t* d_list_cpos;
+    const uint8_t* d_list_code;
+    uint32_t* d_error;                  /* set when a restart marker carries the wrong number */
+    int16_t* d_coef;
+    size_t coef_count;
+    int dequantize;                     /* 1: finish with coefficient * quantiser wrapped to int16 (integer IDCT flavour) */
+    int comp_count;
+    int comp_blk_off[GJ_MAX_COMP];      /* first block of every component (dequantisation table qinv_zz[component]) */
+    const struct gj_dev_dec_tables* d_tables;
+};
+/* zero the coefficients, decode every scan in stream order, dequantise */
+int gj_launch_progressive_decode(const struct gj_prog_args* a, gj_stream_t stream);
 
 /* K0: marker list of the entropy-coded part of the file, built on the device (gj_markers.cu)
  * [replaces ref: src/gpujpeg_reader.c:1038-1155] */

@@ -109,4 +109,12 @@ for kind, q, rst, il, name, samp in content[:2] if quick else content:
     e4.close()
     d4.close()
     print("ok content", kind, q, rst, il, name, flush=True)
+# progressive frames (k_prog_decode, every scan kind, with and without restart markers; dequantisation for the integer IDCT)
+import _progressive as pr  # noqa: E402
+for rst, samp in ((0, (2, 2)), (3, (1, 1))):
+    base, _, prog, _ = pr.twin(o.gen_image("photo", 97, 61), 80, rst, pr.script("libjpeg"), samp)
+    d5 = g.Decoder()
+    assert np.array_equal(d5.decode(prog), o.decode(base)) and np.array_equal(decf.decode(prog), o.decode(base, o.IDCT_FLOAT_GPUREF))
+    d5.close()
+    print("ok progressive", rst, samp, flush=True)
 print("all sanitizer cases ok")
