@@ -80,6 +80,7 @@ struct gpujpeg_decoder {
     uint32_t* d_k3_ctr;                             /* K3 work counters (8 words, zero between launches) */
     uint32_t* h_mk;                                 /* pinned mirror */
     int16_t* d_coef; size_t d_coef_size;
+    uint8_t* d_cext; size_t d_cext_size;     /* one extent byte per block of d_coef (GJ_CEXT_FULL) */
     uint8_t* d_raw; size_t d_raw_size;
     uint8_t* h_raw; size_t h_raw_size;       /* pinned, INTERNAL_BUFFER output */
 
@@ -188,6 +189,7 @@ int gpujpeg_decoder_destroy(struct gpujpeg_decoder* d)
     gj_cuda_free(d->d_k3_ctr);
     gj_cuda_free_host(d->h_mk);
     gj_cuda_free(d->d_coef);
+    gj_cuda_free(d->d_cext);
     gj_cuda_free(d->d_planes);
     gj_cuda_free(d->d_raw);
     gj_cuda_free_host(d->h_raw);
@@ -270,6 +272,7 @@ int gpujpeg_decoder_init(struct gpujpeg_decoder* d, const struct gpujpeg_paramet
     gj_geometry_init(&d->geo, &p, &pi);
     const struct gj_geometry* g = &d->geo;
     if ( grow_dev((void**)&d->d_coef, &d->d_coef_size, g->coef_count * 2) ||
+         grow_dev((void**)&d->d_cext, &d->d_cext_size, g->coef_count / 64) ||
          grow_dev((void**)&d->d_raw, &d->d_raw_size, g->raw_size) ) {
         GJ_ERR("Decoder device allocation failed: %s\n", gj_cuda_last_error());
         return -1;
@@ -359,13 +362,13 @@ static int launch_k4(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], 
 {
     const struct gj_geometry* g = &d->geo;
     if ( d->out_mode == GJ_OUT_SAMPLES )
-        return gj_launch_idct_samples(d->d_coef, g->comp, g->comp_count, comp_tq, d_out, &d->raw, d->idct_flavour,
+        return gj_launch_idct_samples(d->d_coef, d->d_cext, g->comp, g->comp_count, comp_tq, d_out, &d->raw, d->idct_flavour,
                                       coef_dequantized, &d->h_tab, d->stream);
     if ( d->out_mode == GJ_OUT_GENERIC ) {
         struct gj_raw_layout pl;
         struct gj_comp_geo padded[GJ_MAX_COMP];
         gj_planes_layout(&pl, padded, g->comp, g->comp_count);
-        if ( gj_launch_idct_samples(d->d_coef, padded, g->comp_count, comp_tq, d->d_planes, &pl, d->idct_flavour,
+        if ( gj_launch_idct_samples(d->d_coef, d->d_cext, padded, g->comp_count, comp_tq, d->d_planes, &pl, d->idct_flavour,
                                     coef_dequantized, &d->h_tab, d->stream) )
             return -1;
         if ( d->flipped && gj_launch_flip_planes(d->d_planes, padded, g->comp_count, d->stream) ) return -1;
@@ -380,9 +383,9 @@ static int launch_k4(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], 
         pitch = -pitch;
     }
     if ( g->lay.simple )
-        return gj_launch_idct_rgb444(d->d_coef, g->bcx, g->bcy, comp_tq, d_out, g->width, g->height, pitch, d->idct_flavour,
+        return gj_launch_idct_rgb444(d->d_coef, d->d_cext, g->bcx, g->bcy, comp_tq, d_out, g->width, g->height, pitch, d->idct_flavour,
                                      coef_dequantized, &d->h_tab, d->stream);
-    return gj_launch_idct_rgb_ss(d->d_coef, g->comp, comp_tq, d_out, g->width, g->height, pitch, d->idct_flavour,
+    return gj_launch_idct_rgb_ss(d->d_coef, d->d_cext, g->comp, comp_tq, d_out, g->width, g->height, pitch, d->idct_flavour,
                                  coef_dequantized, &d->h_tab, d->stream);
 }
 
@@ -449,9 +452,9 @@ static int decode_striped(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_CO
                 if ( gj_launch_huffman_decode(&part, d->stream) ) return -1;
             }
         }
-        const int rc = g->lay.simple ? gj_launch_idct_rgb444_rows(d->d_coef, g->bcx, g->bcy, my0, my1, comp_tq, d_out, g->width, g->height,
+        const int rc = g->lay.simple ? gj_launch_idct_rgb444_rows(d->d_coef, d->d_cext, g->bcx, g->bcy, my0, my1, comp_tq, d_out, g->width, g->height,
                                                                   g->pitch, d->idct_flavour, coef_dequantized, &d->h_tab, d->stream)
-                                     : gj_launch_idct_rgb_ss_rows(d->d_coef, g->comp, my0, my1, comp_tq, d_out, g->width, g->height, g->pitch,
+                                     : gj_launch_idct_rgb_ss_rows(d->d_coef, d->d_cext, g->comp, my0, my1, comp_tq, d_out, g->width, g->height, g->pitch,
                                                                   d->idct_flavour, coef_dequantized, &d->h_tab, d->stream);
         if ( rc ||
              gj_cuda_event_record(d->ev_stripe[i], d->stream) || gj_cuda_stream_wait_event(d->copy_stream, d->ev_stripe[i]) ||
@@ -936,6 +939,7 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
     a->d_list_code = d->d_list_code;
     a->d_error = d->d_mk + 3;
     a->d_coef = d->d_coef;
+    a->d_cext = d->d_cext;
     a->coef_count = g->coef_count;
     a->dequantize = d->idct_flavour == 0;
     a->comp_count = g->comp_count;
@@ -1224,6 +1228,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     ha.lay = g->lay;
     ha.seg_mcu = g->seg_mcu;
     ha.d_coef = d->d_coef;
+    ha.d_cext = d->d_cext;
     ha.d_tables = d->d_tab;
     d->last_args = ha;
     d->last_ecs_begin = ecs_begin;
@@ -1455,6 +1460,6 @@ GPUJPEG_API int gpujpegx_decoder_run_resident(struct gpujpeg_decoder* d, uint8_t
 GPUJPEG_API int gpujpegx_decoder_get_coefficients(struct gpujpeg_decoder* d, int16_t* out, size_t count)
 {
     if ( !d || !d->initialised || !d->last_valid || count != d->geo.coef_count ) return -1;
-    if ( gj_coef_to_host_natural(d->d_coef, count, out, d->stream) ) return -1;
+    if ( gj_coef_to_host_natural(d->d_coef, d->d_cext, count, out, d->stream) ) return -1;
     return (d->last_progressive ? d->last_prog.dequantize : d->last_args.dequantize) ? 1 : 0;
 }

@@ -60,6 +60,28 @@ GJ_HD constexpr int gj_nat2zz(int n)
 }
 
 /* ------------------------------------------------------------------------------------------- */
+/* block extents between K3 and K4 (format: GJ_CEXT_FULL in gj_internal.h)                       */
+
+/* extent of a block whose last stored coefficient has zig-zag index last_zz (0..63) */
+GJ_HD int gj_cext_of(int last_zz) { return (last_zz >> 3) + 1; }
+/* is zig-zag coefficient k of a block with extent ext stored in the coefficient buffer?  (otherwise it is zero) */
+GJ_HD bool gj_cext_holds(int ext, int k) { return (k >> 3) < ext; }
+
+#if defined(__CUDACC__)
+/* the 64 zig-zag coefficients of a block as 32 packed int16 pairs: chunks below the extent from the buffer, the rest zero.
+ * The loop is unrolled, so the register layout is that of a whole-block load. */
+__device__ __forceinline__ void gj_load_coef_block(const int16_t* __restrict__ blk, int ext, uint32_t (&packed)[32])
+{
+    const uint4* src = reinterpret_cast<const uint4*>(blk);
+#pragma unroll
+    for ( int i = 0; i < 8; i++ ) {
+        const uint4 t = i < ext ? __ldg(src + i) : make_uint4(0u, 0u, 0u, 0u);
+        packed[4 * i] = t.x; packed[4 * i + 1] = t.y; packed[4 * i + 2] = t.z; packed[4 * i + 3] = t.w;
+    }
+}
+#endif
+
+/* ------------------------------------------------------------------------------------------- */
 /* colour transforms                                                                             */
 
 /* RGB -> YCbCr (JPEG full range).  Integer definition [ref: src/gpujpeg_colorspace.h:64-79, 251-266]:

@@ -26,9 +26,10 @@
  * sum per component afterwards (the predictor chain is the one truly sequential thing in a segment).
  *
  * Output: dense scans (at most two segments per warp) stage their blocks in shared memory and flush whole 128-byte
- * lines; sparse scans (many short segments per warp, a handful of non-zeros per block) zero-fill their blocks in
- * global memory and store the non-zeros directly.  Either way every coefficient of every block is written: no
- * memset of the 200 MB coefficient buffer.
+ * lines; sparse scans (many short segments per warp, a handful of non-zeros per block) stage the first 16 coefficients
+ * of every block, zero-fill the rest of it in global memory and store the non-zeros there directly.  Every block also
+ * gets its extent byte (GJ_CEXT_FULL): 8 for a staged block, 2 for a split one unless a value landed past zig-zag 15,
+ * then 8.  No memset of the 200 MB coefficient buffer.
  *
  * Semantics follow the reference decoders: garbage codes read as "end of block" / DC size 0
  * (src/gpujpeg_huffman_gpu_decoder.cu:565-577, src/gpujpeg_huffman_cpu_decoder.c:155-159), the predictor is reset at
@@ -86,6 +87,7 @@ struct SdParams {
     int warm_x8;                                 // warm-up of a sub-sequence's first walk, in eighths of an average block
     uint32_t* error;
     int16_t* coef;
+    uint8_t* cext;                       // block extents (GJ_CEXT_FULL)
     const gj_dev_dec_tables* tables;
 };
 
@@ -377,7 +379,7 @@ struct StageStride { static constexpr int value = MODE == M_STAGED ? 64 : SD_HEA
 template <bool DEQ, bool IL, int MODE, bool SM>
 __device__ __forceinline__ void walk_write(const Walk& W, uint32_t st, uint32_t p_end, int n, int nblocks,
                                            const uint32_t* __restrict__ tgt, int16_t* __restrict__ stage,
-                                           int16_t* __restrict__ glob, int16_t* __restrict__ coef)
+                                           int16_t* __restrict__ glob, int16_t* __restrict__ coef, uint8_t* __restrict__ ext)
 {
     uint32_t k = (st >> 18) & 127u, c = st >> 25;
     const uint32_t p = st & 0x3FFFFu;
@@ -409,7 +411,10 @@ __device__ __forceinline__ void walk_write(const Walk& W, uint32_t st, uint32_t 
         else if ( size && idx < 64u ) {
             const int16_t dv = (int16_t)(DEQ ? v * (int)qt[idx] : v);
             if ( MODE == M_SPLIT && idx < (uint32_t)SD_HEAD ) so[idx] = dv;
-            else o[idx] = dv;
+            else {
+                o[idx] = dv;
+                if ( MODE == M_SPLIT ) ext[!IL ? n : (int)tgt[n]] = GJ_CEXT_FULL;
+            }
         }
         q += total;
         k += kadv;
@@ -432,7 +437,7 @@ __device__ __forceinline__ void walk_write(const Walk& W, uint32_t st, uint32_t 
 template <bool DEQ, bool IL, int MODE>
 __device__ __forceinline__ void walk_write_sm(const Walk& W, uint32_t st, uint32_t p_end, int n, int nblocks,
                                               const uint32_t* __restrict__ tgt, int16_t* __restrict__ stage,
-                                              int16_t* __restrict__ glob, int16_t* __restrict__ coef)
+                                              int16_t* __restrict__ glob, int16_t* __restrict__ coef, uint8_t* __restrict__ ext)
 {
     uint32_t c = st >> 25;
     const uint32_t p = st & 0x3FFFFu;
@@ -465,7 +470,10 @@ __device__ __forceinline__ void walk_write_sm(const Walk& W, uint32_t st, uint32
         if ( pend ) {
             const int dv = DEQ ? pend_v * (int)pend_q : pend_v;
             if ( MODE == M_STAGED || pend_at < SS ) sts16(pend_sb + 2u * pend_at, (uint32_t)dv);
-            else g_out[pend_gb + pend_at] = (int16_t)dv;
+            else {
+                g_out[pend_gb + pend_at] = (int16_t)dv;
+                ext[pend_gb >> 6] = GJ_CEXT_FULL;
+            }
         }
     };
     while ( S < S_end ) {
@@ -599,6 +607,7 @@ __device__ __forceinline__ void run_units(const SdParams& P, const int scan, con
         }
         /* first block of the segment in the coefficient buffer (one scan per component: its blocks are consecutive) */
         int16_t* const seg_glob = IL ? P.coef : P.coef + ((size_t)L.blk_off[scan] + first_mcu) * 64;
+        uint8_t* const seg_ext = IL ? P.cext : P.cext + (size_t)L.blk_off[scan] + first_mcu;   // indexed as seg_glob, per block
         if ( IL ) {
             for ( int j = gl; j < nblocks; j += lanes )
                 tgt[j] = block_target(L, scan, first_mcu, j);
@@ -608,6 +617,11 @@ __device__ __forceinline__ void run_units(const SdParams& P, const int scan, con
 
         auto body = [&](auto sm_tag) {
             constexpr bool SM = decltype(sm_tag)::value;
+            /* the extents of the segment's blocks: a staged block is whole; a split block is its staged head unless the
+             * writing walk stores a value past it (that walk raises the extent to GJ_CEXT_FULL; the tail is zero-filled
+             * below either way, so the extent never has to be found before the values are written) */
+            for ( int j = gl; j < nblocks; j += lanes )
+                seg_ext[IL ? (int)tgt[j] : j] = MODE == M_STAGED ? GJ_CEXT_FULL : SD_HEAD / 8;
             if ( MODE == M_SPLIT ) {
                 /* zero the part of every block that is not staged: uint4 number 2..7 of its eight.  Four stores per round
                  * with addresses of their own: a store holds its address registers until the memory pipe has taken it
@@ -629,7 +643,7 @@ __device__ __forceinline__ void run_units(const SdParams& P, const int scan, con
                 }
                 for ( ; i < n16; i += lanes )
                     zero_at(i);
-                __syncwarp();   // the zeros are in place before any lane stores a value into the same block
+                __syncwarp();   // the zeros and extents are in place before any lane stores a value into the same block
             }
 
             /* ---- sub-sequences: one per lane of the segment's group ---- */
@@ -673,8 +687,8 @@ __device__ __forceinline__ void run_units(const SdParams& P, const int scan, con
 
             /* ---- the walk that writes ---- */
             if ( active ) {
-                if constexpr ( SM ) walk_write_sm<DEQ, IL, MODE>(W, start, p_end, n0, nblocks, tgt, seg_stage, seg_glob, P.coef);
-                else walk_write<DEQ, IL, MODE, false>(W, start, p_end, n0, nblocks, tgt, seg_stage, seg_glob, P.coef);
+                if constexpr ( SM ) walk_write_sm<DEQ, IL, MODE>(W, start, p_end, n0, nblocks, tgt, seg_stage, seg_glob, P.coef, seg_ext);
+                else walk_write<DEQ, IL, MODE, false>(W, start, p_end, n0, nblocks, tgt, seg_stage, seg_glob, P.coef, seg_ext);
             }
         };
         if ( fits ) body(std::true_type{});
@@ -887,6 +901,7 @@ extern "C" int gj_launch_huffman_decode_sync(const struct gj_huff_dec_args* a, g
     P.seg_mcu = a->seg_mcu;
     P.error = a->d_error;
     P.coef = a->d_coef;
+    P.cext = a->d_cext;
     P.tables = a->d_tables;
     const int segblk = a->seg_mcu * a->lay.bpm;
     int total_units = 0, max_spu_tgt = 0;

@@ -19,8 +19,9 @@
  * DECODER (replaces src/gpujpeg_huffman_gpu_decoder.cu:390-537, 596-610):
  *   k_huff_decode   one THREAD per restart segment (sequential by nature); the owner lanes of a warp advance
  *                   block by block in lock step, each decoding into a private shared-memory block that
- *                   the whole warp then writes out as 128-byte lines (no memset of the coefficient
- *                   buffer, no scattered 2-byte stores).  Tables: 9-bit lookahead + canonical
+ *                   the whole warp then writes out as 128-byte lines, and the block's extent byte
+ *                   (GJ_CEXT_FULL) next to it (no memset of the coefficient buffer, no scattered 2-byte
+ *                   stores).  Tables: 9-bit lookahead + canonical
  *                   bounds (1.4 KB per table) instead of the reference's 4 x 64 Ki-entry tables.
  *
  * Scans, segments and the block order inside them (4:4:4 or subsampled, interleaved or not) come from the
@@ -997,7 +998,7 @@ template <bool DEQ>
 __global__ void __launch_bounds__(HD_THREADS)
 k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file_end, const uint32_t* __restrict__ seg_off,
               int seg_count, int seg_mcu, const __grid_constant__ gj_huff_dec_args a, const __grid_constant__ SegOwners own,
-              int16_t* __restrict__ coef, const gj_dev_dec_tables* __restrict__ tables)
+              int16_t* __restrict__ coef, uint8_t* __restrict__ cext, const gj_dev_dec_tables* __restrict__ tables)
 {
     gj_pdl_wait();
     __shared__ DecTabs s_tab;
@@ -1089,6 +1090,7 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
     for ( int b = 0; b < max_blocks; b++ ) {
         /* ci: position of the block's component in the scan header (tables, predictor) */
         const int ci = general ? L.idx_comp[bi_in_mcu] : bi_in_mcu;
+        int ext = 0;   // extent of this lane's block (GJ_CEXT_FULL)
         if ( live && !absent && b < nblocks ) {
             const gj_dec_lut& tdc = s_tab.t[0][a.scan_td[scan][ci]];
             const gj_dec_lut& tac = s_tab.t[1][a.scan_ta[scan][ci]];
@@ -1104,7 +1106,8 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
             else if ( ci == 2 ) pr = (pred[2] += diff);
             else pr = (pred[3] += diff);
             mine[(0 ^ sw) << 3] = (int16_t)(DEQ ? pr * (int)q[0] : pr);
-            for ( int k = 1; k < 64; ) {
+            int k = 1;
+            while ( k < 64 ) {
                 src_fill(r);
                 const int rs = decode_symbol(r, tac);
                 const int run = rs >> 4;
@@ -1120,6 +1123,9 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
                     k += 16;                 // ZRL
                 }
             }
+            /* k is one past the last coefficient stored, or past a run of zeros behind it (a ZRL before EOB): then the
+             * extent is larger than needed, which is exact too, as the whole block is written below */
+            ext = gj_cext_of(min(k, 64) - 1);
         }
         __syncwarp();
         /* where this lane's block goes (index in units of 64 coefficients) */
@@ -1132,6 +1138,8 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
         else {
             target = mybase + (L.interleaved ? L.blk_off[a.scan_comp[0][ci]] : 0) + mcu;
         }
+        /* the block's extent (absent segments: 0, the block is zero) */
+        if ( live && b < nblocks ) cext[target] = (uint8_t)ext;
         /* write the warp's SPW private blocks out as 128-byte lines, four blocks per step, and clear them */
         for ( int j = 0; j < SPW / 4; j++ ) {
             const int i = 4 * j + (lane >> 3);   // owner lane of the block this lane helps to move
@@ -1160,12 +1168,13 @@ __constant__ uint8_t c_zz2nat[64] = {
     0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
     41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
     30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
-__global__ void k_coef_to_natural(const int16_t* __restrict__ in, int16_t* __restrict__ out, size_t nblocks)
+__global__ void k_coef_to_natural(const int16_t* __restrict__ in, const uint8_t* __restrict__ cext, int16_t* __restrict__ out,
+                                  size_t nblocks)
 {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if ( i >= nblocks * 64 ) return;
     const int k = (int)(i & 63);
-    out[(i & ~(size_t)63) + c_zz2nat[k]] = in[i];
+    out[(i & ~(size_t)63) + c_zz2nat[k]] = !cext || gj_cext_holds(cext[i >> 6], k) ? in[i] : (int16_t)0;
 }
 
 }  // namespace
@@ -1311,19 +1320,19 @@ extern "C" int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_str
     const dim3 grid((warps + HD_THREADS / 32 - 1) / (HD_THREADS / 32));
     if ( a->dequantize )
         gj_launch_pdl(k_huff_decode<true>, dim3(grid), dim3(HD_THREADS), 0, stream, a->d_file, a->d_file + a->file_size, a->d_seg_off,
-                      a->seg_count, a->seg_mcu, *a, own, a->d_coef, a->d_tables);
+                      a->seg_count, a->seg_mcu, *a, own, a->d_coef, a->d_cext, a->d_tables);
     else
         gj_launch_pdl(k_huff_decode<false>, dim3(grid), dim3(HD_THREADS), 0, stream, a->d_file, a->d_file + a->file_size, a->d_seg_off,
-                      a->seg_count, a->seg_mcu, *a, own, a->d_coef, a->d_tables);
+                      a->seg_count, a->seg_mcu, *a, own, a->d_coef, a->d_cext, a->d_tables);
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
-extern "C" int gj_coef_to_host_natural(const int16_t* d_coef, size_t count, int16_t* h_out, gj_stream_t stream)
+extern "C" int gj_coef_to_host_natural(const int16_t* d_coef, const uint8_t* d_cext, size_t count, int16_t* h_out, gj_stream_t stream)
 {
     int16_t* d_tmp = nullptr;
     if ( cudaMalloc(&d_tmp, count * sizeof(int16_t)) != cudaSuccess ) return -1;
     const size_t nblocks = count / 64;
-    k_coef_to_natural<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(d_coef, d_tmp, nblocks);
+    k_coef_to_natural<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(d_coef, d_cext, d_tmp, nblocks);
     cudaMemcpyAsync(h_out, d_tmp, count * sizeof(int16_t), cudaMemcpyDeviceToHost, stream);
     const cudaError_t e = cudaStreamSynchronize(stream);
     cudaFree(d_tmp);

@@ -309,17 +309,17 @@ int gj_launch_fdct_rgb444(const uint8_t* d_raw, int width, int height, int pitch
 /* block rows [by0, by1) of the frame only: the stripe pipelines of the host-buffer calls (gj_encoder.c, gj_decoder.c) */
 int gj_launch_fdct_rgb444_rows(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
                                int bcx, int bcy, int by0, int by1, const struct gj_dev_enc_tables* d_tables, gj_stream_t stream);
-int gj_launch_idct_rgb444_rows(const int16_t* d_coef, int bcx, int bcy, int by0, int by1, const int comp_tq[3], uint8_t* d_raw,
-                               int width, int height, int pitch, int idct_flavour, int coef_dequantized,
-                               const struct gj_dev_dec_tables* d_tables, gj_stream_t stream);
+int gj_launch_idct_rgb444_rows(const int16_t* d_coef, const uint8_t* d_cext, int bcx, int bcy, int by0, int by1,
+                               const int comp_tq[3], uint8_t* d_raw, int width, int height, int pitch, int idct_flavour,
+                               int coef_dequantized, const struct gj_dev_dec_tables* d_tables, gj_stream_t stream);
 
 /* the same for the chroma-subsampled kernels: MCU rows [my0, my1), an MCU row = 8 * comp[0].vs image rows */
 int gj_launch_fdct_rgb_ss_rows(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
                                const struct gj_comp_geo comp[3], int my0, int my1, const struct gj_dev_enc_tables* h_tables,
                                gj_stream_t stream);
-int gj_launch_idct_rgb_ss_rows(const int16_t* d_coef, const struct gj_comp_geo comp[3], int my0, int my1, const int comp_tq[3],
-                               uint8_t* d_raw, int width, int height, int pitch, int idct_flavour, int coef_dequantized,
-                               const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
+int gj_launch_idct_rgb_ss_rows(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], int my0, int my1,
+                               const int comp_tq[3], uint8_t* d_raw, int width, int height, int pitch, int idct_flavour,
+                               int coef_dequantized, const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
 
 /* K2: Huffman-encode every restart segment and assemble the finished scan data
  * [replaces ref: src/gpujpeg_huffman_gpu_encoder.cu:1071-1167 + host loop src/gpujpeg_encoder.c:567-626]
@@ -359,7 +359,15 @@ int gj_launch_huffman_place(const struct gj_huff_enc_args* a, gj_stream_t stream
 #define GJ_HUFF_COUNTS_BYTES (2 * 2 * 256 * sizeof(uint64_t))
 int gj_launch_huffman_stats(const struct gj_huff_enc_args* a, uint64_t* d_counts, gj_stream_t stream);
 
-/* K3: Huffman-decode every restart segment into zig-zag coefficients
+/* Block extent, the decoder's format between K3 and K4: next to its coefficient buffer the decoder keeps one byte per
+ * 64-coefficient block, at the block's index in the coefficient buffer.  Its value n (0..GJ_CEXT_FULL) says that the
+ * 16-byte chunks 0..n-1 of the block (chunk i = zig-zag coefficients 8i..8i+7) are valid in the coefficient buffer and
+ * that every coefficient past them is zero, whatever the buffer holds there.  Every decode path writes the extent of
+ * every block of the frame on every frame, blocks it leaves zero included, so that chunks a denser earlier frame left
+ * behind are never read.  Helpers: gj_cext_of, gj_load_coef_block (gj_device.cuh). */
+#define GJ_CEXT_FULL 8
+
+/* K3: Huffman-decode every restart segment into zig-zag coefficients and block extents
  * [replaces ref: src/gpujpeg_huffman_gpu_decoder.cu:663-746] */
 struct gj_huff_dec_args {
     const uint8_t* d_file;      /* the JPEG bytes */
@@ -399,6 +407,7 @@ struct gj_huff_dec_args {
     int scan_td[GJ_MAX_COMP][GJ_MAX_COMP], scan_ta[GJ_MAX_COMP][GJ_MAX_COMP];
     int scan_tq[GJ_MAX_COMP][GJ_MAX_COMP]; /* quantisation table id of that component */
     int16_t* d_coef;
+    uint8_t* d_cext;            /* the extent of every block of d_coef (GJ_CEXT_FULL) */
     const struct gj_dev_dec_tables* d_tables;
 };
 int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_stream_t stream);
@@ -434,6 +443,7 @@ struct gj_prog_args {
     const uint8_t* d_list_code;
     uint32_t* d_error;                  /* set when a restart marker carries the wrong number */
     int16_t* d_coef;
+    uint8_t* d_cext;                    /* block extents: all GJ_CEXT_FULL (the scans accumulate into the dense buffer) */
     size_t coef_count;
     int dequantize;                     /* 1: finish with coefficient * quantiser wrapped to int16 (integer IDCT flavour) */
     int comp_count;
@@ -449,11 +459,11 @@ int gj_launch_marker_scan(const uint8_t* d_file, size_t begin, size_t end, unsig
                           uint8_t* d_list_code, uint32_t* d_list_cpos, uint32_t list_cap, uint8_t* d_clean, uint32_t* d_result,
                           uint32_t* d_other, uint32_t other_cap, gj_stream_t stream);
 
-/* K4: zig-zag coefficients -> RGB u8 interleaved (fused dequant + IDCT + colour transform)
+/* K4: zig-zag coefficients and their block extents -> RGB u8 interleaved (fused dequant + IDCT + colour transform)
  * idct_flavour: 0 = integer (gpujpeg_idct_cpu), 1 = float GPU-reference
  * [replaces ref: src/gpujpeg_dct_gpu.cu:681-727 + src/gpujpeg_postprocessor.cu:444-496] */
-int gj_launch_idct_rgb444(const int16_t* d_coef, int bcx, int bcy, const int comp_tq[3], uint8_t* d_raw, int width,
-                          int height, int pitch, int idct_flavour, int coef_dequantized,
+int gj_launch_idct_rgb444(const int16_t* d_coef, const uint8_t* d_cext, int bcx, int bcy, const int comp_tq[3], uint8_t* d_raw,
+                          int width, int height, int pitch, int idct_flavour, int coef_dequantized,
                           const struct gj_dev_dec_tables* d_tables, gj_stream_t stream);
 
 /* K1 / K4 for chroma-subsampled streams: luminance comp[0].hs x comp[0].vs in {2x1, 2x2, 1x2}, chrominance 1x1
@@ -461,8 +471,8 @@ int gj_launch_idct_rgb444(const int16_t* d_coef, int bcx, int bcy, const int com
  *  src/gpujpeg_postprocessor.cu:271-282 plus the DCT launches] */
 int gj_launch_fdct_rgb_ss(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
                           const struct gj_comp_geo comp[3], const struct gj_dev_enc_tables* h_tables, gj_stream_t stream);
-int gj_launch_idct_rgb_ss(const int16_t* d_coef, const struct gj_comp_geo comp[3], const int comp_tq[3], uint8_t* d_raw,
-                          int width, int height, int pitch, int idct_flavour, int coef_dequantized,
+int gj_launch_idct_rgb_ss(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], const int comp_tq[3],
+                          uint8_t* d_raw, int width, int height, int pitch, int idct_flavour, int coef_dequantized,
                           const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
 
 /* K1 / K4 without colour transform, any pixel format gj_raw_layout_init describes, any sampling: one thread per 8x8
@@ -472,8 +482,8 @@ int gj_launch_idct_rgb_ss(const int16_t* d_coef, const struct gj_comp_geo comp[3
 int gj_launch_fdct_samples(const uint8_t* d_raw, const struct gj_raw_layout* raw, int16_t* d_coef, uint64_t* d_nzmask,
                            const struct gj_comp_geo* comp, int comp_count, const uint8_t* comp_tbl,
                            const struct gj_dev_enc_tables* h_tables, gj_stream_t stream);
-int gj_launch_idct_samples(const int16_t* d_coef, const struct gj_comp_geo* comp, int comp_count, const int* comp_tq,
-                           uint8_t* d_raw, const struct gj_raw_layout* raw, int idct_flavour, int coef_dequantized,
+int gj_launch_idct_samples(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
+                           const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int idct_flavour, int coef_dequantized,
                            const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
 
 /* Generic pre-/post-processing pass (gj_convert.cu): raw image in any supported pixel format and colour space <-> the
@@ -499,8 +509,9 @@ int gj_parse_bool(const char* val, const char* optname);
 void gj_planes_layout(struct gj_raw_layout* l, struct gj_comp_geo padded[GJ_MAX_COMP], const struct gj_comp_geo* comp,
                       int comp_count);
 
-/* debug/test helper: device coefficient buffer (zig-zag) -> host natural order, block-major */
-int gj_coef_to_host_natural(const int16_t* d_coef, size_t count, int16_t* h_out, gj_stream_t stream);
+/* debug/test helper: device coefficient buffer (zig-zag) -> host natural order, block-major; coefficients past a block's
+ * extent read as zero (d_cext NULL: every block is whole, as the encoder's) */
+int gj_coef_to_host_natural(const int16_t* d_coef, const uint8_t* d_cext, size_t count, int16_t* h_out, gj_stream_t stream);
 
 /* thin wrappers over the CUDA runtime so the host files stay plain C without cuda headers */
 int gj_cuda_malloc(void** p, size_t size);

@@ -6,8 +6,9 @@
  * end-of-band runs over blocks) and AC refinements (one more bit of a band: correction bits for coefficients that are
  * non-zero already, run/sign for the ones that become non-zero).  Each scan reads and extends what the earlier scans left.
  *
- *   k_prog_zero  the coefficient buffer starts at zero (blocks no scan reaches stay zero): an ordinary launch behind the
- *                table upload, and a kernel, so that the first scan kernel can depend on it programmatically
+ *   k_prog_zero  the coefficient buffer starts at zero (blocks no scan reaches stay zero) and every block's extent at
+ *                GJ_CEXT_FULL (the scans accumulate into the dense buffer): an ordinary launch behind the table upload,
+ *                and a kernel, so that the first scan kernel can depend on it programmatically
  *   k_prog_decode<KIND>   one launch per scan, in stream order, chained with programmatic dependent launch: one THREAD
  *                per restart segment, reading K0's clean stream (segment bounds from the marker list, as K3); the
  *                per-block logic is gj_prog_segment in gj_device.cuh, which the CPU tests run as well
@@ -53,10 +54,12 @@ k_prog_decode(const __grid_constant__ gj_prog_scan S, const gj_dec_lut* __restri
     gj_prog_segment<KIND>(S, s_tab, clean, cs, ce > cs ? ce : cs, s, coef);
 }
 
-__global__ void __launch_bounds__(DQ_THREADS) k_prog_zero(uint4* __restrict__ p, size_t n16)
+__global__ void __launch_bounds__(DQ_THREADS) k_prog_zero(uint4* __restrict__ p, size_t n16, uint8_t* __restrict__ cext)
 {
-    for ( size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (size_t)gridDim.x * blockDim.x )
+    for ( size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (size_t)gridDim.x * blockDim.x ) {
         p[i] = make_uint4(0u, 0u, 0u, 0u);
+        if ( (i & 7) == 0 ) cext[i >> 3] = GJ_CEXT_FULL;
+    }
 }
 
 struct DqComps {
@@ -85,7 +88,7 @@ extern "C" int gj_launch_progressive_decode(const struct gj_prog_args* a, gj_str
     {   /* (coef_count is a multiple of 64: whole blocks of 128 bytes) */
         const size_t n16 = a->coef_count / 8;
         const size_t blocks = (n16 + DQ_THREADS - 1) / DQ_THREADS;
-        k_prog_zero<<<(unsigned)(blocks < cap ? blocks : cap), DQ_THREADS, 0, stream>>>(reinterpret_cast<uint4*>(a->d_coef), n16);
+        k_prog_zero<<<(unsigned)(blocks < cap ? blocks : cap), DQ_THREADS, 0, stream>>>(reinterpret_cast<uint4*>(a->d_coef), n16, a->d_cext);
         if ( cudaGetLastError() != cudaSuccess ) return -1;
     }
     for ( int k = 0; k < a->scan_count; k++ ) {
