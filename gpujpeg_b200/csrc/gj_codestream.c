@@ -84,19 +84,19 @@ int gj_raw_layout_init(struct gj_raw_layout* l, const struct gpujpeg_image_param
 }
 
 void gj_planes_layout(struct gj_raw_layout* l, struct gj_comp_geo padded[GJ_MAX_COMP], const struct gj_comp_geo* comp,
-                      int comp_count)
+                      int comp_count, int n)
 {
     memset(l, 0, sizeof *l);
     l->comp_count = comp_count;
     for ( int c = 0; c < comp_count; c++ ) {
-        l->comp[c] = (struct gj_raw_comp){(size_t)comp[c].blk_off * 64, (size_t)comp[c].bcx * 8, 1};
+        l->comp[c] = (struct gj_raw_comp){(size_t)comp[c].blk_off * n * n, (size_t)comp[c].bcx * n, 1};
         l->sampling[c].horizontal = (uint8_t)comp[c].hs;
         l->sampling[c].vertical = (uint8_t)comp[c].vs;
-        l->size = ((size_t)comp[c].blk_off + comp[c].nblk) * 64;
-        /* the planes are padded to whole blocks with zeros: treat the padding as samples, every row is 8-byte aligned */
+        l->size = ((size_t)comp[c].blk_off + comp[c].nblk) * n * n;
+        /* the planes are padded to whole blocks with zeros: treat the padding as samples (n = 8: every row is 8-byte aligned) */
         padded[c] = comp[c];
-        padded[c].width = comp[c].bcx * 8;
-        padded[c].height = comp[c].bcy * 8;
+        padded[c].width = comp[c].bcx * n;
+        padded[c].height = comp[c].bcy * n;
     }
 }
 

@@ -30,7 +30,7 @@ struct ConvertParams {
     int raw_comps;          /* 1: grey */
     int uyvy;               /* 422-u8-p1020: U is stored by even pixels, V by odd pixels */
     int alpha_off;          /* 4444-u8-p0123: offset of the alpha byte inside a pixel, 0 = none */
-    /* component planes of the JPEG: sample (x, y) of component c at poff + y * ppitch + x; a pixel contributes to /
+    /* component planes of the JPEG (n samples per block side): sample (x, y) of component c at poff + y * ppitch + x; a pixel contributes to /
      * reads from plane c at (x / pdh, y / pdv).  A fourth component is the alpha of a 4444-u8-p0123 image: it passes by
      * the colour transform [ref: src/gpujpeg_preprocessor.cu:131-138, src/gpujpeg_postprocessor.cu:122-131] */
     unsigned long long poff[GJ_MAX_COMP];
@@ -158,7 +158,7 @@ k_channel_remap(uint8_t* __restrict__ raw, const __grid_constant__ RemapParams p
 
 int fill_params(ConvertParams* p, const struct gj_raw_layout* raw, enum gpujpeg_pixel_format fmt, int color_space,
                 int color_space_internal, int width, int height, const struct gj_comp_geo* comp, int comp_count, int max_hs,
-                int max_vs)
+                int max_vs, int n)
 {
     memset(p, 0, sizeof *p);
     if ( color_space_internal < GPUJPEG_RGB || color_space_internal > GPUJPEG_YCBCR_BT709 ) return -1;
@@ -179,8 +179,8 @@ int fill_params(ConvertParams* p, const struct gj_raw_layout* raw, enum gpujpeg_
     }
     for ( int k = 0; k < GJ_MAX_COMP; k++ ) {
         const int j = k < comp_count ? k : 0;
-        p->poff[k] = (unsigned long long)comp[j].blk_off * 64;
-        p->ppitch[k] = comp[j].bcx * 8;
+        p->poff[k] = (unsigned long long)comp[j].blk_off * n * n;
+        p->ppitch[k] = comp[j].bcx * n;
         p->pdh[k] = max_hs / comp[j].hs;
         p->pdv[k] = max_vs / comp[j].vs;
     }
@@ -199,7 +199,7 @@ extern "C" int gj_launch_convert_in(const uint8_t* d_raw, const struct gj_raw_la
                                     gj_stream_t stream)
 {
     ConvertParams p;
-    if ( fill_params(&p, raw, fmt, color_space, color_space_internal, width, height, comp, comp_count, max_hs, max_vs) ) return -1;
+    if ( fill_params(&p, raw, fmt, color_space, color_space_internal, width, height, comp, comp_count, max_hs, max_vs, 8) ) return -1;
     if ( comp_count == 4 && !raw->alpha_off ) return -1;   /* a fourth component needs a pixel format that has alpha samples */
     /* samples outside the image are 0 [ref: src/gpujpeg_common.c:941-944] */
     if ( cudaMemsetAsync(d_planes, 0, planes_size, stream) != cudaSuccess ) return -1;
@@ -209,11 +209,11 @@ extern "C" int gj_launch_convert_in(const uint8_t* d_raw, const struct gj_raw_la
 
 extern "C" int gj_launch_convert_out(const uint8_t* d_planes, uint8_t* d_raw, const struct gj_raw_layout* raw,
                                      enum gpujpeg_pixel_format fmt, int color_space, int color_space_internal, int width,
-                                     int height, const struct gj_comp_geo* comp, int comp_count, int max_hs, int max_vs,
+                                     int height, const struct gj_comp_geo* comp, int comp_count, int max_hs, int max_vs, int n,
                                      gj_stream_t stream)
 {
     ConvertParams p;
-    if ( fill_params(&p, raw, fmt, color_space, color_space_internal, width, height, comp, comp_count, max_hs, max_vs) ) return -1;
+    if ( fill_params(&p, raw, fmt, color_space, color_space_internal, width, height, comp, comp_count, max_hs, max_vs, n) ) return -1;
     k_convert_out<<<dim3((width + 255) / 256, height), 256, 0, stream>>>(d_planes, d_raw, p);
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -805,6 +805,48 @@ k_idct_samples(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cex
     }
 }
 
+/* Scaled decoding (dec_opt_scale): libjpeg's reduced IDCT (gj_idct_scaled_block), N x N samples per block, one thread per
+ * block as k_idct_samples.  The coefficients are the raw quantised values; they are dequantised here in 32 bits.  Only the
+ * chunks below the block's extent are loaded (at N = 1 only the DC); g.cw / g.ch count samples of the scaled component. */
+template <int N>
+__global__ void __launch_bounds__(SG_THREADS)
+k_idct_scaled(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext, const __grid_constant__ SampleGrid g, int total_blocks,
+              uint8_t* __restrict__ raw, const __grid_constant__ IdctParams prm)
+{
+    const int bi = blockIdx.x * SG_THREADS + threadIdx.x;
+    if ( bi >= total_blocks ) return;
+    const int comp = (bi >= g.blk_off[1]) + (bi >= g.blk_off[2]) + (bi >= g.blk_off[3]);
+    const int local = bi - g.blk_off[comp];
+    const int by = local / g.bcx[comp], bx = local - by * g.bcx[comp];
+    const int vw = min(N, g.cw[comp] - bx * N), vh = min(N, g.ch[comp] - by * N);
+    if ( vw <= 0 || vh <= 0 ) return;
+    const uint16_t* q = prm.q_zz[comp];
+    const int ext = __ldg(cext + bi);
+    int v[64];
+    if ( N == 1 ) {
+        v[0] = ext > 0 ? (int)((uint32_t)(int)__ldg(coef + (size_t)bi * 64) * (uint32_t)q[0]) : 0;
+    }
+    else {
+        uint32_t packed[32];
+        gj_load_coef_block(coef + (size_t)bi * 64, ext, packed);
+#pragma unroll
+        for ( int k = 0; k < 64; k++ ) {
+            const int c = (k & 1) ? (int)packed[k >> 1] >> 16 : (int)(short)(packed[k >> 1] & 0xFFFFu);
+            v[gj_zz2nat(k)] = (int)((uint32_t)c * (uint32_t)q[k]);
+        }
+    }
+    int px[N * N];
+    gj_idct_scaled_block<N>(v, px);
+    uint8_t* dst = raw + g.off[comp] + (size_t)by * N * g.pitch[comp] + (size_t)bx * N * g.xs[comp];
+#pragma unroll
+    for ( int y = 0; y < N; y++ ) {
+        if ( y >= vh ) continue;
+#pragma unroll
+        for ( int x = 0; x < N; x++ )
+            if ( x < vw ) dst[(size_t)y * g.pitch[comp] + (size_t)x * g.xs[comp]] = (uint8_t)px[N * y + x];
+    }
+}
+
 int pick_vec(const void* p, size_t pitch)
 {
     const uintptr_t a = reinterpret_cast<uintptr_t>(p) | pitch;
@@ -1090,5 +1132,23 @@ extern "C" int gj_launch_idct_samples(const int16_t* d_coef, const uint8_t* d_ce
         k_idct_samples<0, true><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
     else
         k_idct_samples<1, true><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
+    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+extern "C" int gj_launch_idct_scaled(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
+                                     const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int n,
+                                     const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
+{
+    IdctParams prm;
+    for ( int c = 0; c < GJ_MAX_COMP; c++ )
+        memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c < comp_count ? c : 0]], sizeof prm.q_zz[c]);
+    SampleGrid sg;
+    const int total = sample_grid(&sg, raw, comp, comp_count, nullptr);
+    if ( total <= 0 ) return -1;
+    const int grid = (total + SG_THREADS - 1) / SG_THREADS;
+    if ( n == 4 ) k_idct_scaled<4><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
+    else if ( n == 2 ) k_idct_scaled<2><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
+    else if ( n == 1 ) k_idct_scaled<1><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
+    else return -1;
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

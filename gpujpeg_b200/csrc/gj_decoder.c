@@ -59,7 +59,14 @@ struct gpujpeg_decoder {
     int ff_cs_itu601_is_709;      /* [ref: libgpujpeg/gpujpeg_decoder.h:95] */
     int out_mode;                 /* GJ_OUT_RGB, GJ_OUT_SAMPLES or GJ_OUT_GENERIC: which K4 runs */
     uint8_t* d_planes; size_t d_planes_size;   /* component planes between the IDCT and the generic pass */
-    struct gj_raw_layout raw;     /* where the samples go (GJ_OUT_SAMPLES) */
+    struct gj_raw_layout raw;     /* where the samples go (GJ_OUT_SAMPLES; every output of a scaled frame) */
+    /* scaled decoding (dec_opt_scale): scale_req is the option, scale the divisor of the frame being / last decoded (1, 2, 4
+     * or 8); the frame's output is out_w x out_h pixels, out_size bytes; scomp = the component planes at that scale (the
+     * block grids of geo.comp, 8 / scale samples per block side, width / height the samples that carry image data) */
+    int scale_req, scale;
+    int out_w, out_h;
+    size_t out_size;
+    struct gj_comp_geo scomp[GJ_MAX_COMP];
     struct gpujpeg_image_metadata metadata;
 
     struct gj_dev_dec_tables h_tab, h_tab_prev;
@@ -152,6 +159,7 @@ struct gpujpeg_decoder* gpujpeg_decoder_create_with_params(const struct gpujpeg_
     d->sm_count = gj_cuda_sm_count();
     d->req_pixel_format = GPUJPEG_PIXFMT_AUTODETECT;
     d->k3_parts = -1;
+    d->scale_req = d->scale = 1;
     d->req_color_space = GPUJPEG_CS_DEFAULT;
     if ( d->device < 0 || gj_cuda_malloc((void**)&d->d_tab, sizeof *d->d_tab) ||
          gj_cuda_malloc((void**)&d->d_mk, GJ_MK_WORDS * 4 + GJ_CTA_BYTES0) || gj_cuda_malloc((void**)&d->d_k3_ctr, 32) ||
@@ -271,9 +279,10 @@ int gpujpeg_decoder_init(struct gpujpeg_decoder* d, const struct gpujpeg_paramet
         pi.pixel_format = p.comp_count == 1 ? GPUJPEG_U8 : p.comp_count == 4 ? GPUJPEG_4444_U8_P0123 : GPUJPEG_444_U8_P012;
     gj_geometry_init(&d->geo, &p, &pi);
     const struct gj_geometry* g = &d->geo;
+    /* (the output of a scaled frame is smaller: gpujpeg_decoder_decode sizes d_raw for it, size_output) */
     if ( grow_dev((void**)&d->d_coef, &d->d_coef_size, g->coef_count * 2) ||
          grow_dev((void**)&d->d_cext, &d->d_cext_size, g->coef_count / 64) ||
-         grow_dev((void**)&d->d_raw, &d->d_raw_size, g->raw_size) ) {
+         (d->scale == 1 && grow_dev((void**)&d->d_raw, &d->d_raw_size, g->raw_size)) ) {
         GJ_ERR("Decoder device allocation failed: %s\n", gj_cuda_last_error());
         return -1;
     }
@@ -357,24 +366,43 @@ static int choose_output(const struct gpujpeg_decoder* d, const struct gj_stream
     return GJ_OUT_SAMPLES;
 }
 
+/* K4 of a scaled frame: the reduced IDCT straight into the output (GJ_OUT_SAMPLES) or into component planes of 8 / scale
+ * samples per block side that the generic pass turns into the output */
+static int launch_k4_scaled(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], uint8_t* d_out)
+{
+    const struct gj_geometry* g = &d->geo;
+    const int n = 8 / d->scale;
+    if ( d->out_mode == GJ_OUT_SAMPLES )
+        return gj_launch_idct_scaled(d->d_coef, d->d_cext, d->scomp, g->comp_count, comp_tq, d_out, &d->raw, n, &d->h_tab, d->stream);
+    struct gj_raw_layout pl;
+    struct gj_comp_geo padded[GJ_MAX_COMP];
+    gj_planes_layout(&pl, padded, g->comp, g->comp_count, n);
+    if ( gj_launch_idct_scaled(d->d_coef, d->d_cext, padded, g->comp_count, comp_tq, d->d_planes, &pl, n, &d->h_tab, d->stream) )
+        return -1;
+    return gj_launch_convert_out(d->d_planes, d_out, &d->raw, d->param_image.pixel_format, d->param_image.color_space,
+                                 d->param.color_space_internal, d->out_w, d->out_h, g->comp, g->comp_count, g->max_hs, g->max_vs, n,
+                                 d->stream);
+}
+
 /* K4 for the coder's geometry: the 4:4:4 kernel or the chroma-subsampling template instance */
 static int launch_k4(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], uint8_t* d_out, int coef_dequantized)
 {
     const struct gj_geometry* g = &d->geo;
+    if ( d->scale > 1 ) return launch_k4_scaled(d, comp_tq, d_out);
     if ( d->out_mode == GJ_OUT_SAMPLES )
         return gj_launch_idct_samples(d->d_coef, d->d_cext, g->comp, g->comp_count, comp_tq, d_out, &d->raw, d->idct_flavour,
                                       coef_dequantized, &d->h_tab, d->stream);
     if ( d->out_mode == GJ_OUT_GENERIC ) {
         struct gj_raw_layout pl;
         struct gj_comp_geo padded[GJ_MAX_COMP];
-        gj_planes_layout(&pl, padded, g->comp, g->comp_count);
+        gj_planes_layout(&pl, padded, g->comp, g->comp_count, 8);
         if ( gj_launch_idct_samples(d->d_coef, d->d_cext, padded, g->comp_count, comp_tq, d->d_planes, &pl, d->idct_flavour,
                                     coef_dequantized, &d->h_tab, d->stream) )
             return -1;
         if ( d->flipped && gj_launch_flip_planes(d->d_planes, padded, g->comp_count, d->stream) ) return -1;
         return gj_launch_convert_out(d->d_planes, d_out, &d->raw, d->param_image.pixel_format, d->param_image.color_space,
                                      d->param.color_space_internal,
-                                     g->width, g->height, g->comp, g->comp_count, g->max_hs, g->max_vs, d->stream);
+                                     g->width, g->height, g->comp, g->comp_count, g->max_hs, g->max_vs, 8, d->stream);
     }
     /* dec_opt_flipped on the fused path (see gpujpeg_decoder_decode): rows are written last to first */
     int pitch = g->pitch;
@@ -389,7 +417,8 @@ static int launch_k4(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], 
                                  coef_dequantized, &d->h_tab, d->stream);
 }
 
-/* The stripe pipeline applies to what the fused RGB kernels write as they go: no flip, no channel remap. */
+/* The stripe pipeline applies to what the fused RGB kernels write as they go: no flip, no channel remap (and no scaled
+ * frame: those never take GJ_OUT_RGB). */
 static int stripes_usable(struct gpujpeg_decoder* d)
 {
     const struct gj_geometry* g = &d->geo;
@@ -743,7 +772,6 @@ static int upload_file(struct gpujpeg_decoder* d, const uint8_t* image, size_t i
 static int k4_and_output(struct gpujpeg_decoder* d, struct gpujpeg_decoder_output* output, const struct gpujpeg_image_parameters* pi,
                          const int comp_tq[GJ_MAX_COMP], int dequantize, int striped, const struct gj_huff_dec_args* k3_part, int stats)
 {
-    const struct gj_geometry* g = &d->geo;
     const int to_host = output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER || output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_BUFFER;
     uint8_t* d_out = d->d_raw;
     if ( output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_CUDA_BUFFER ) {
@@ -757,7 +785,7 @@ static int k4_and_output(struct gpujpeg_decoder* d, struct gpujpeg_decoder_outpu
     uint8_t* h_dst = output->data;
     if ( to_host ) {
         if ( output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER ) {
-            if ( grow_host((void**)&d->h_raw, &d->h_raw_size, g->raw_size) ) return -1;
+            if ( grow_host((void**)&d->h_raw, &d->h_raw_size, d->out_size) ) return -1;
             h_dst = d->h_raw;
         }
         else if ( !h_dst ) {
@@ -790,12 +818,12 @@ static int k4_and_output(struct gpujpeg_decoder* d, struct gpujpeg_decoder_outpu
         gj_timer_stop(&d->t_gpu, d->stream);
     }
 
-    output->data_size = g->raw_size;
+    output->data_size = d->out_size;
     output->param_image = *pi;
     if ( to_host ) {
         if ( !copied ) {
             if ( stats && d->timers_ok ) gj_timer_start(&d->t_from, d->stream);
-            if ( gj_cuda_memcpy_d2h_async(h_dst, d_out, g->raw_size, d->stream) ) {
+            if ( gj_cuda_memcpy_d2h_async(h_dst, d_out, d->out_size, d->stream) ) {
                 GJ_ERR("Decoder copy of raw data failed: %s\n", gj_cuda_last_error());
                 return -1;
             }
@@ -838,6 +866,30 @@ static void record_stats(struct gpujpeg_decoder* d, const struct gpujpeg_decoder
     }
 }
 
+/* The output buffers of the frame: pi is the output (at scaled frames ceil(W / scale) x ceil(H / scale) pixels), d->geo the
+ * stream's own geometry.  A scaled component keeps its block grid; its samples that carry image data are counted as
+ * gj_geometry_init counts them for an image of the output's size. */
+static int size_output(struct gpujpeg_decoder* d, const struct gpujpeg_image_parameters* pi)
+{
+    const struct gj_geometry* g = &d->geo;
+    const int n = 8 / d->scale;
+    d->out_w = pi->width;
+    d->out_h = pi->height;
+    d->out_size = d->scale == 1 ? g->raw_size : d->raw.size;
+    for ( int c = 0; c < g->comp_count; c++ ) {
+        const int div_h = g->max_hs / g->comp[c].hs, div_v = g->max_vs / g->comp[c].vs;
+        d->scomp[c] = g->comp[c];
+        d->scomp[c].width = (pi->width + div_h - 1) / div_h;
+        d->scomp[c].height = (pi->height + div_v - 1) / div_v;
+    }
+    if ( grow_dev((void**)&d->d_raw, &d->d_raw_size, d->out_size) ||
+         (d->out_mode == GJ_OUT_GENERIC && grow_dev((void**)&d->d_planes, &d->d_planes_size, g->coef_count / 64 * n * n)) ) {
+        GJ_ERR("Decoder device allocation failed: %s\n", gj_cuda_last_error());
+        return -1;
+    }
+    return 0;
+}
+
 /* Progressive (SOF2) frames, from the first SOS on: the same upload, K0 and host marker walk as a baseline frame, then per
  * scan the parameters and Huffman tables (those in force at its SOS), one table upload, the scan kernels in stream order
  * (gj_progressive.cu) and the same K4 / output stage.  Segment-info tables and dec_opt_huffman / dec_opt_huffman_lanes do not
@@ -877,9 +929,11 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
     for ( int k = 0; k < st->scan_count; k++ )
         il |= st->scan[k].ncomp > 1;
     if ( il != p->interleaved ) {
+        struct gpujpeg_image_parameters pg = *pi;   /* the coefficient planes: the stream's own size */
+        pg.width = st->width;
+        pg.height = st->height;
         p->interleaved = il;
-        if ( gpujpeg_decoder_init(d, p, pi) ) return GPUJPEG_ERROR;
-        if ( d->out_mode == GJ_OUT_GENERIC && grow_dev((void**)&d->d_planes, &d->d_planes_size, d->geo.coef_count) ) return GPUJPEG_ERROR;
+        if ( gpujpeg_decoder_init(d, p, &pg) || size_output(d, pi) ) return GPUJPEG_ERROR;
     }
     const struct gj_geometry* g = &d->geo;
 
@@ -941,7 +995,7 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
     a->d_coef = d->d_coef;
     a->d_cext = d->d_cext;
     a->coef_count = g->coef_count;
-    a->dequantize = d->idct_flavour == 0;
+    a->dequantize = d->idct_flavour == 0 && d->scale == 1;   /* the reduced IDCT dequantises the raw values itself */
     a->comp_count = g->comp_count;
     for ( int c = 0; c < g->comp_count; c++ )
         a->comp_blk_off[c] = g->comp[c].blk_off;
@@ -1044,12 +1098,23 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     const enum gpujpeg_color_space early_cs = gj_stream_color_space(&st, adobe);
     st.color_space = early_cs;
     p.color_space_internal = early_cs;
+    /* dec_opt_scale: the output is ceil(W / scale) x ceil(H / scale) pixels, negotiated as a full-size image of that size */
+    if ( d->scale_req > 1 && d->flipped ) {
+        GJ_ERR("dec_opt_flipped is not supported together with dec_opt_scale.\n");
+        return GPUJPEG_ERROR;
+    }
+    if ( d->scale != d->scale_req ) d->last_valid = 0;   /* a resident re-run must not mix the buffers of two scales */
+    d->scale = d->scale_req;
     struct gpujpeg_image_parameters pi;
     gpujpeg_image_set_default_parameters(&pi);
-    pi.width = st.width;
-    pi.height = st.height;
+    pi.width = (st.width + d->scale - 1) / d->scale;
+    pi.height = (st.height + d->scale - 1) / d->scale;
     int out_mode = choose_output(d, &st, &pi);
     if ( !out_mode ) return GPUJPEG_ERROR;
+    if ( d->scale > 1 && out_mode == GJ_OUT_RGB ) out_mode = GJ_OUT_GENERIC;   /* the fused kernels are full-size only */
+    struct gpujpeg_image_parameters pg = pi;   /* the coefficient planes: the stream's own size */
+    pg.width = st.width;
+    pg.height = st.height;
     /* the flip acts on the component planes, padding included, in front of the postprocessor
      * [ref: src/gpujpeg_postprocessor.cu:447]: in general only the pass that has planes can do it.  Without vertical padding
      * flipping the planes and then replicating chrominance rows is flipping the finished image, and the fused kernel does
@@ -1057,18 +1122,17 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     if ( d->flipped && !(out_mode == GJ_OUT_RGB && st.height % (8 * (st.comp_count >= 3 ? (st.comp_hv[0] & 15) : 1)) == 0) )
         out_mode = GJ_OUT_GENERIC;
 
-    if ( !d->initialised || d->param_image.width != pi.width || d->param_image.height != pi.height ||
-         d->param_image.pixel_format != pi.pixel_format || d->param.comp_count != p.comp_count ||
+    if ( !d->initialised || d->param_image.width != pg.width || d->param_image.height != pg.height ||
+         d->param_image.pixel_format != pg.pixel_format || d->param.comp_count != p.comp_count ||
          d->param.color_space_internal != p.color_space_internal ||
          d->param.restart_interval != p.restart_interval || d->param.interleaved != p.interleaved ||
          memcmp(d->param.sampling_factor, p.sampling_factor, sizeof p.sampling_factor) != 0 ) {
         if ( d->initialised ) GJ_VERBOSE(d->verbose, "Reinitializing decoder.\n");
-        if ( gpujpeg_decoder_init(d, &p, &pi) ) return GPUJPEG_ERROR;
+        if ( gpujpeg_decoder_init(d, &p, &pg) ) return GPUJPEG_ERROR;
     }
     d->out_mode = out_mode;
     d->param_image.color_space = pi.color_space;
-    if ( out_mode != GJ_OUT_RGB && gj_raw_layout_init(&d->raw, &pi) ) return GPUJPEG_ERROR;
-    if ( out_mode == GJ_OUT_GENERIC && grow_dev((void**)&d->d_planes, &d->d_planes_size, d->geo.coef_count) ) return GPUJPEG_ERROR;
+    if ( (out_mode != GJ_OUT_RGB && gj_raw_layout_init(&d->raw, &pi)) || size_output(d, &pi) ) return GPUJPEG_ERROR;
     const struct gj_geometry* g = &d->geo;
 
     if ( st.progressive ) return decode_progressive(d, image, image_size, output, &st, &p, &pi, pos, adobe, early_cs, stats, t_begin);
@@ -1191,7 +1255,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     /* ---- K3 ---- */
     ha.d_file = d->d_file;
     ha.file_size = image_size;
-    ha.dequantize = d->idct_flavour == 0;
+    ha.dequantize = d->idct_flavour == 0 && d->scale == 1;   /* the reduced IDCT dequantises the raw values itself */
     ha.d_seg_off = by_table ? d->d_seg_off : NULL; /* segment starts: the stream's own table, or the device-built marker list */
     ha.d_seg_len = NULL;
     ha.d_list_pos = d->d_list_pos;
@@ -1406,6 +1470,16 @@ int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt,
         decoder->channel_remap = m;
         return GPUJPEG_NOERR;
     }
+    if ( strcmp(opt, GPUJPEG_DEC_OPT_SCALE) == 0 ) {
+        static const char* const vals[4] = {"1", "1/2", "1/4", "1/8"};
+        for ( int i = 0; i < 4; i++ )
+            if ( strcmp(val, vals[i]) == 0 ) {
+                decoder->scale_req = 1 << i;
+                return GPUJPEG_NOERR;
+            }
+        GJ_ERR("Unknown decoding scale: %s (1, 1/2, 1/4 or 1/8)\n", val);
+        return GPUJPEG_ERROR;
+    }
     if ( strcmp(opt, GPUJPEG_DEC_OPT_TGA_RLE_BOOL) == 0 || strcmp(opt, GPUJPEG_DEC_OPT_ALIGNMENT_BYTES_INT) == 0 ) {
         GJ_ERR("Decoder option %s is not implemented in this build.\n", opt);
         return GPUJPEG_ERROR;
@@ -1420,6 +1494,8 @@ void gpujpeg_decoder_print_options(void)
            "] - inverse DCT flavour (default: int = gpujpeg_idct_cpu)\n");
     printf("\t" GPUJPEG_DEC_OPT_FLIPPED_BOOL "=[" GPUJPEG_VAL_FALSE "|" GPUJPEG_VAL_TRUE "] - flip the decoded image vertically\n");
     printf("\t" GPUJPEG_DEC_OPT_CHANNEL_REMAP "=XYZ[W] - output channel mapping (as the encoder option)\n");
+    printf("\t" GPUJPEG_DEC_OPT_SCALE "=[1|1/2|1/4|1/8] - decode to ceil(W*scale) x ceil(H*scale) pixels with libjpeg's reduced inverse "
+           "DCTs (default: 1)\n");
 }
 
 GPUJPEG_API int gpujpegx_decoder_used_segment_info(const struct gpujpeg_decoder* d)

@@ -411,6 +411,87 @@ GJ_HD void gj_idct_float_block(float (&f)[64])
 }
 
 /* ------------------------------------------------------------------------------------------- */
+/* reduced inverse DCTs of scaled decoding (dec_opt_scale) == libjpeg's jidctred.c                */
+/* (jpeg_idct_4x4, jpeg_idct_2x2, jpeg_idct_1x1: CONST_BITS 13, PASS1_BITS 2)                       */
+/* Input: the RAW quantised coefficient times its quantiser, natural order, as 32-bit integers (not the int16-wrapped product
+ * the integer flavour of K3 stores).  Every sum and product wraps in 32 bits; that is libjpeg's arithmetic wherever no
+ * intermediate leaves 31 bits, which holds for everything an 8-bit encoder writes.  The zero-column / zero-row shortcuts of
+ * jidctred.c give the same values as the full formulas and are left out.  Output: N x N samples, row-major, 0..255. */
+
+/* DESCALE(x, n) with an arithmetic shift, on the wrapped value */
+GJ_HD int gj_red_descale(uint32_t x, int n) { return (int)(x + (1u << (n - 1))) >> n; }
+/* libjpeg's range-limit table, indexed by v & 1023 (RANGE_MASK) after the +128 centre */
+GJ_HD int gj_red_limit(int v)
+{
+    const int m = v & 1023;
+    return m < 128 ? m + 128 : m < 512 ? 255 : m < 896 ? 0 : m - 896;
+}
+/* one 4-point pass of jpeg_idct_4x4 (input 4 is not used); x0 << 14 is the even part's DC term */
+GJ_HD void gj_red4(uint32_t x0, uint32_t x1, uint32_t x2, uint32_t x3, uint32_t x5, uint32_t x6, uint32_t x7, int shift, int& o0,
+                   int& o1, int& o2, int& o3)
+{
+    const uint32_t e0 = x0 << 14, e2 = x2 * 15137u - x6 * 6270u;
+    const uint32_t t10 = e0 + e2, t12 = e0 - e2;
+    const uint32_t t0 = x1 * 8697u - x3 * 17799u + x5 * 11893u - x7 * 1730u;
+    const uint32_t t2 = x1 * 20995u + x3 * 7373u - x5 * 4926u - x7 * 4176u;
+    o0 = gj_red_descale(t10 + t2, shift);
+    o3 = gj_red_descale(t10 - t2, shift);
+    o1 = gj_red_descale(t12 + t0, shift);
+    o2 = gj_red_descale(t12 - t0, shift);
+}
+/* one 2-point pass of jpeg_idct_2x2 (inputs 0, 1, 3, 5, 7) */
+GJ_HD void gj_red2(uint32_t x0, uint32_t x1, uint32_t x3, uint32_t x5, uint32_t x7, int shift, int& o0, int& o1)
+{
+    const uint32_t t10 = x0 << 15;
+    const uint32_t t0 = x1 * 29692u - x3 * 10426u + x5 * 6967u - x7 * 5906u;
+    o0 = gj_red_descale(t10 + t0, shift);
+    o1 = gj_red_descale(t10 - t0, shift);
+}
+/* N = 4 (scale 1/2), 2 (1/4) or 1 (1/8).  Coefficients the transform does not read may hold anything. */
+template <int N>
+GJ_HD void gj_idct_scaled_block(const int (&in)[64], int (&out)[N * N])
+{
+    if ( N == 1 ) {
+        out[0] = gj_red_limit(gj_red_descale((uint32_t)in[0], 3));
+    }
+    else if ( N == 2 ) {
+        int ws[2][8];   /* columns 0, 1, 3, 5, 7 (the row pass reads no other) */
+#pragma unroll
+        for ( int c = 0; c < 8; c++ ) {
+            if ( c == 2 || c == 4 || c == 6 ) continue;
+            gj_red2((uint32_t)in[c], (uint32_t)in[8 + c], (uint32_t)in[24 + c], (uint32_t)in[40 + c], (uint32_t)in[56 + c], 13,
+                    ws[0][c], ws[1][c]);
+        }
+#pragma unroll
+        for ( int r = 0; r < 2; r++ ) {
+            int a, b;
+            gj_red2((uint32_t)ws[r][0], (uint32_t)ws[r][1], (uint32_t)ws[r][3], (uint32_t)ws[r][5], (uint32_t)ws[r][7], 20, a, b);
+            out[N * r] = gj_red_limit(a);
+            out[N * r + 1] = gj_red_limit(b);
+        }
+    }
+    else {
+        int ws[4][8];   /* every column but 4 */
+#pragma unroll
+        for ( int c = 0; c < 8; c++ ) {
+            if ( c == 4 ) continue;
+            gj_red4((uint32_t)in[c], (uint32_t)in[8 + c], (uint32_t)in[16 + c], (uint32_t)in[24 + c], (uint32_t)in[40 + c],
+                    (uint32_t)in[48 + c], (uint32_t)in[56 + c], 12, ws[0][c], ws[1][c], ws[2][c], ws[3][c]);
+        }
+#pragma unroll
+        for ( int r = 0; r < 4; r++ ) {
+            int a, b, c, d;
+            gj_red4((uint32_t)ws[r][0], (uint32_t)ws[r][1], (uint32_t)ws[r][2], (uint32_t)ws[r][3], (uint32_t)ws[r][5],
+                    (uint32_t)ws[r][6], (uint32_t)ws[r][7], 19, a, b, c, d);
+            out[N * r] = gj_red_limit(a);
+            out[N * r + 1] = gj_red_limit(b);
+            out[N * r + 2] = gj_red_limit(c);
+            out[N * r + 3] = gj_red_limit(d);
+        }
+    }
+}
+
+/* ------------------------------------------------------------------------------------------- */
 /* Huffman helpers                                                                               */
 
 /* number of significant bits of |v| (JPEG "category")  [ref: src/gpujpeg_huffman_cpu_encoder.c:159-164] */

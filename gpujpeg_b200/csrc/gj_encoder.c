@@ -336,7 +336,7 @@ static int launch_k1(struct gpujpeg_encoder* e, const uint8_t* d_raw)
     if ( e->input_mode == GJ_IN_GENERIC ) {
         struct gj_raw_layout pl;
         struct gj_comp_geo padded[GJ_MAX_COMP];
-        gj_planes_layout(&pl, padded, g->comp, g->comp_count);
+        gj_planes_layout(&pl, padded, g->comp, g->comp_count, 8);
         if ( gj_launch_convert_in(d_raw, &e->raw, e->param_image.pixel_format, e->param_image.color_space,
                                   e->param.color_space_internal, g->width, g->height,
                                   e->d_planes, pl.size, g->comp, g->comp_count, g->max_hs, g->max_vs, e->stream) )

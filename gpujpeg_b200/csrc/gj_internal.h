@@ -485,16 +485,22 @@ int gj_launch_fdct_samples(const uint8_t* d_raw, const struct gj_raw_layout* raw
 int gj_launch_idct_samples(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
                            const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int idct_flavour, int coef_dequantized,
                            const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
+/* K4 of scaled decoding (dec_opt_scale): libjpeg's reduced inverse DCT, n = 4, 2 or 1 samples per block side (scale 1/2, 1/4,
+ * 1/8), from RAW quantised coefficients; comp[c].width / height are the component's sample extents at that scale */
+int gj_launch_idct_scaled(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
+                          const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int n,
+                          const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
 
 /* Generic pre-/post-processing pass (gj_convert.cu): raw image in any supported pixel format and colour space <-> the
- * component planes of the YCbCr JPEG (plane c at byte comp[c].blk_off * 64, pitch comp[c].bcx * 8)
+ * component planes of the YCbCr JPEG (plane c at byte comp[c].blk_off * n * n, pitch comp[c].bcx * n, n samples per block
+ * side: 8, or fewer for the planes of a scaled decode)
  * [replaces the generic kernels of ref: src/gpujpeg_preprocessor.cu:163-201, src/gpujpeg_postprocessor.cu:183-216] */
 int gj_launch_convert_in(const uint8_t* d_raw, const struct gj_raw_layout* raw, enum gpujpeg_pixel_format fmt, int color_space,
                          int color_space_internal, int width, int height, uint8_t* d_planes, size_t planes_size,
                          const struct gj_comp_geo* comp, int comp_count, int max_hs, int max_vs, gj_stream_t stream);
 int gj_launch_convert_out(const uint8_t* d_planes, uint8_t* d_raw, const struct gj_raw_layout* raw, enum gpujpeg_pixel_format fmt,
                           int color_space, int color_space_internal, int width, int height, const struct gj_comp_geo* comp,
-                          int comp_count, int max_hs, int max_vs, gj_stream_t stream);
+                          int comp_count, int max_hs, int max_vs, int n, gj_stream_t stream);
 /* enc/dec_opt_flipped: vertical flip of the (padded) component planes; enc/dec_opt_channel_remap: channel permutation of
  * the raw image in place.  gj_launch_channel_remap returns -2 when the channel count does not match the pixel format and
  * -3 for pixel formats with chroma subsampling [replaces ref: src/gpujpeg_preprocessor.cu:456-559] */
@@ -505,9 +511,9 @@ int gj_launch_channel_remap(uint8_t* d_raw, const struct gj_raw_layout* raw, enu
 unsigned gj_parse_channel_remap(const char* val, const char* optname);
 /* "1" / "0" / "true" / "false" ... -> 0 / 1, -1 on error [ref: src/gpujpeg_common.c gpujpeg_parse_bool_opt] */
 int gj_parse_bool(const char* val, const char* optname);
-/* the planes above described as a raw layout, so that the sample kernels can run on them */
+/* the planes above described as a raw layout, so that the sample kernels can run on them (n samples per block side) */
 void gj_planes_layout(struct gj_raw_layout* l, struct gj_comp_geo padded[GJ_MAX_COMP], const struct gj_comp_geo* comp,
-                      int comp_count);
+                      int comp_count, int n);
 
 /* debug/test helper: device coefficient buffer (zig-zag) -> host natural order, block-major; coefficients past a block's
  * extent read as zero (d_cext NULL: every block is whole, as the encoder's) */

@@ -486,6 +486,13 @@ GPUJPEG_API int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size
 /* extension (tuning): lanes that share one restart segment in the self-synchronising decoder: 0 = chosen per scan from
  * the scan's bytes per segment (default), or 4, 8, 16, 32 for every scan */
 #define GPUJPEG_DEC_OPT_HUFFMAN_LANES "dec_opt_huffman_lanes"
+/* Extension of this build (not in the reference): scaled decoding.  "1" (default), "1/2", "1/4" or "1/8": the decoder
+ * returns an image of ceil(W / s) x ceil(H / s) pixels (in output->param_image and data_size, for every output type),
+ * computed with libjpeg's reduced inverse DCTs (jidctred.c: jpeg_idct_4x4, jpeg_idct_2x2, jpeg_idct_1x1) from the raw
+ * quantised coefficients; chrominance is replicated and colour-converted as at full size.  dec_opt_idct does not apply to
+ * scaled frames (there is one arithmetic); dec_opt_flipped together with a scale is refused.  gpujpeg_decoder_get_image_info
+ * still reports the stream's own size. */
+#define GPUJPEG_DEC_OPT_SCALE "dec_opt_scale"
 GPUJPEG_API int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt, const char* val);
 GPUJPEG_API void gpujpeg_decoder_print_options(void);
 
