@@ -890,6 +890,7 @@ constexpr int HD_THREADS = 128;
 #endif
 /* segment owners per warp: fewer for frames with fewer segments (profiles/k3_matrix.py times the choices) */
 constexpr int HD_SEGMENTS_PER_WARP = GJ_HD_SPW;
+constexpr size_t HD_CMP_MAX = 12 * 1024;   // bytes of clean stream staged per warp at most (4 warps: 48 KB besides the static tables)
 
 struct DecTabs {
     gj_dec_lut t[2][4];
@@ -956,14 +957,47 @@ __device__ __forceinline__ void src_fill(BitSource& r)
         }
     }
 }
-__device__ __forceinline__ uint32_t src_peek16(const BitSource& r) { return (uint32_t)(r.acc >> (r.n - 16)) & 0xFFFFu; }
-__device__ __forceinline__ uint32_t src_get(BitSource& r, int len)
+/* Bit source of one lane on K0's clean stream (stuffing, fill bytes and markers already removed; big-endian words): the
+ * words of the warp's segments staged in shared memory, or the clean stream in global memory when they do not fit -- a
+ * generic pointer serves both.  One word is fetched ahead.  Past the segment's last word and three more it reads zeros,
+ * so a damaged segment never reads outside the words its warp staged. */
+struct CleanSource {
+    const uint32_t* wp;   // next word to fetch
+    const uint32_t* wend; // first word that is not read
+    uint32_t nextw;
+    uint64_t acc;
+    int n;
+};
+__device__ __forceinline__ void src_init(CleanSource& r, const uint32_t* w, const uint32_t* wend, uint32_t bit0)
+{
+    r.wend = wend;
+    r.acc = *w;
+    r.n = 32 - (int)bit0;
+    r.nextw = w[1];
+    r.wp = w + 2;
+}
+/* at least 33 bits available: one word is always enough (no stuffing left to remove) */
+__device__ __forceinline__ void src_fill(CleanSource& r)
+{
+    if ( r.n <= 32 ) {
+        r.acc = (r.acc << 32) | r.nextw;
+        r.n += 32;
+        r.nextw = r.wp < r.wend ? *r.wp : 0u;
+        r.wp++;
+    }
+}
+
+template <class Src>
+__device__ __forceinline__ uint32_t src_peek16(const Src& r) { return (uint32_t)(r.acc >> (r.n - 16)) & 0xFFFFu; }
+template <class Src>
+__device__ __forceinline__ uint32_t src_get(Src& r, int len)
 {
     r.n -= len;
     return (uint32_t)(r.acc >> r.n) & ((1u << len) - 1u);
 }
 
-__device__ __forceinline__ int decode_symbol(BitSource& r, const gj_dec_lut& t)
+template <class Src>
+__device__ __forceinline__ int decode_symbol(Src& r, const gj_dec_lut& t)
 {
     const uint32_t peek = src_peek16(r);
     const uint32_t e = t.look[peek >> (16 - GJ_DEC_LOOK_BITS)];
@@ -988,13 +1022,14 @@ struct SegOwners {
     int segs0;     // segments [0, segs0) use spw0 owners per warp, the rest spw1
     int warps0;    // warps that take segments [0, segs0)
     int spw0, spw1;
+    int cmp_words;   // per warp: words of the clean-stream staging area (dynamic shared memory); 0: read the file bytes
 };
 
 /* SPW = segments per warp: only the first SPW lanes of a warp own a segment, the others just help to move the finished
  * blocks out.  Fewer owners per warp make the warp's instruction stream shorter (the lock-step block loop runs as
  * long as its slowest lane, and every rarely-taken path is executed whenever ANY lane takes it), and that stream,
  * not the issue rate, is what bounds this kernel: 43 200 segments cannot fill the machine anyway. */
-template <bool DEQ>
+template <bool DEQ, bool CLEAN>
 __global__ void __launch_bounds__(HD_THREADS)
 k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file_end, const uint32_t* __restrict__ seg_off,
               int seg_count, int seg_mcu, const __grid_constant__ gj_huff_dec_args a, const __grid_constant__ SegOwners own,
@@ -1034,6 +1069,7 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
     }
     if ( g0 >= g_end ) return;
     if ( !seg_off && !a.d_seg_tab && *a.d_error ) return;   // restart structure does not match the geometry: list ranks are meaningless
+    constexpr bool clean = CLEAN;   // segment positions from K0's marker list, bits from its clean stream (own.cmp_words > 0)
     const int g = g0 + lane;
     const bool live = lane < SPW && g < g_end;
     const gj_scan_layout& L = a.lay;
@@ -1041,8 +1077,7 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
     const bool general = !L.simple && L.interleaved;   // MCUs of several blocks per component
     int scan = 0, nblocks = 0, mybase = 0;
     int mx = 0, my = 0;   // general layout: position of the lane's current MCU
-    BitSource r;
-    r.n = 0;
+    uint32_t start = 0, cs = 0, ce = 0;   // file offset / clean byte range of the lane's segment
     bool absent = false;
     if ( live ) {
         scan = scan_of_segment(L, g);
@@ -1055,7 +1090,6 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
             my = (s * seg_mcu) / L.mcu_x;
             mx = s * seg_mcu - my * L.mcu_x;
         }
-        uint32_t start;
         if ( a.d_seg_tab ) {   // resynchronised stream: explicit table, 0xFFFFFFFF = the segment does not exist (zero blocks)
             start = a.d_seg_tab[3 * (size_t)g];
             absent = start == 0xFFFFFFFFu;
@@ -1076,7 +1110,12 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
             if ( a.d_list_code[m] != (uint8_t)(0xD0 + ((s - 1) & 7)) ) atomicExch(a.d_error, 1u);
         }
         if ( start >= (uint32_t)(file_end - file) ) start = 0;   // corrupt table: stay inside the buffer
-        src_init(r, file + start, file_end);
+        if ( clean ) {
+            const uint32_t r = a.first_rank[scan] + (uint32_t)s;   // the marker that ends the segment
+            ce = a.d_list_cpos[r];
+            cs = s ? a.d_list_cpos[r - 1] : a.scan_cbegin[scan];
+            if ( ce < cs ) ce = cs;
+        }
     }
     const int max_blocks = seg_mcu * bpm;
     /* private block: 16-byte chunk c of lane L lives at chunk (c ^ (L & 7)) so that the warp-wide
@@ -1086,6 +1125,7 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
     uint4* wbase = reinterpret_cast<uint4*>(s_blk + warp * 32 * 32);
     int pred[GJ_MAX_COMP] = {0, 0, 0, 0};
 
+    auto decode_blocks = [&](auto& r) {
     int mcu = 0, bi_in_mcu = 0;   // block b = mcu * bpm + bi_in_mcu, the same in every lane
     for ( int b = 0; b < max_blocks; b++ ) {
         /* ci: position of the block's component in the scan header (tables, predictor) */
@@ -1160,6 +1200,37 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
                 my++;
             }
         }
+    }
+    };
+    if constexpr ( CLEAN ) {
+        /* the warp's segments follow each other in the clean stream: their words -> shared memory with coalesced 16-byte
+         * loads when they fit (the file-byte walk waited for a global load at nearly every refill: the scoreboard tracks
+         * registers per warp, so one lane's refill stalls the lanes that refill an iteration later) */
+        extern __shared__ __align__(16) uint32_t s_cmp_all[];
+        uint32_t* const s_cmp = s_cmp_all + warp * own.cmp_words;
+        const uint32_t lo = __reduce_min_sync(FULL, live ? cs : 0xFFFFFFFFu);
+        const uint32_t hi = __reduce_max_sync(FULL, live ? ce : 0u);
+        const uint32_t wbase = (lo >> 2) & ~3u;
+        const uint32_t need = ((hi + 3u) >> 2) - wbase + 8u;   // + slack: the source reads up to four words past a segment
+        const bool staged = lo <= hi && need <= (uint32_t)own.cmp_words;
+        if ( staged ) {
+            const uint4* src = reinterpret_cast<const uint4*>(a.d_clean + wbase);
+            uint4* dst = reinterpret_cast<uint4*>(s_cmp);
+            for ( uint32_t i = lane; i < (need + 3u) >> 2; i += 32 )
+                dst[i] = __ldg(src + i);
+        }
+        __syncwarp();
+        const uint32_t* w = staged ? s_cmp + ((cs >> 2) - wbase) : a.d_clean + (cs >> 2);
+        CleanSource c;
+        c.n = 0;
+        if ( live ) src_init(c, w, w + ((ce >> 2) - (cs >> 2)) + 4, (cs & 3u) * 8u);
+        decode_blocks(c);
+    }
+    else {
+        BitSource r;
+        r.n = 0;
+        if ( live ) src_init(r, file + start, file_end);
+        decode_blocks(r);
     }
 }
 
@@ -1318,12 +1389,46 @@ extern "C" int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_str
     own.warps0 = (own.segs0 + own.spw0 - 1) / own.spw0;
     const int warps = own.warps0 + (a->seg_count - own.segs0 + own.spw1 - 1) / own.spw1;
     const dim3 grid((warps + HD_THREADS / 32 - 1) / (HD_THREADS / 32));
-    if ( a->dequantize )
-        gj_launch_pdl(k_huff_decode<true>, dim3(grid), dim3(HD_THREADS), 0, stream, a->d_file, a->d_file + a->file_size, a->d_seg_off,
+    /* bits from K0's clean stream wherever the segment positions come from its marker list and the frame is not dense: a
+     * warp's segments staged in shared memory, the area 1.25 times the densest scan's average per warp (more would cost
+     * CTAs per SM: 8K needs five per SM for one wave), a warp whose bytes do not fit reads the clean stream in global
+     * memory.  8K S-photo q75: K3 207 -> 174 us (H100 80GB HBM3, 400 W) */
+    own.cmp_words = 0;
+    if ( !a->d_seg_off && !a->d_seg_tab && a->d_clean && a->d_list_cpos ) {
+        size_t cmp_bytes = 0;
+        for ( int s = 0; s < a->lay.scan_count; s++ ) {
+            const int segs = a->lay.scan_seg_begin[s + 1] - a->lay.scan_seg_begin[s];
+            const int spw = s < 1 || own.segs0 == a->seg_count ? own.spw0 : own.spw1;
+            const size_t want = ((size_t)a->scan_bytes[s] / (size_t)(segs > 0 ? segs : 1) + 16) * (size_t)spw * 5 / 4 + 64;
+            if ( want > cmp_bytes ) cmp_bytes = want;
+        }
+        /* denser frames keep the file bytes: an area that large would cost more resident CTAs than the staging saves
+         * (8K S-random: K3 1333 instead of 665 us) */
+        own.cmp_words = cmp_bytes > HD_CMP_MAX ? 0 : (int)((cmp_bytes + 15) / 16) * 4;
+    }
+    const size_t smem = (size_t)(HD_THREADS / 32) * (size_t)own.cmp_words * 4;
+    /* static tables and blocks + the staging area can exceed the 48 KB a kernel gets without asking */
+    static int attr_done[64];   // 0 = not yet; set once per device (benign if two threads race: same value)
+    int dev = 0;
+    if ( cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 ) return -1;
+    if ( !__atomic_load_n(&attr_done[dev], __ATOMIC_ACQUIRE) ) {
+        if ( cudaFuncSetAttribute(k_huff_decode<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(HD_THREADS / 32 * HD_CMP_MAX + 64)) != cudaSuccess ||
+             cudaFuncSetAttribute(k_huff_decode<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(HD_THREADS / 32 * HD_CMP_MAX + 64)) != cudaSuccess )
+            return -1;
+        __atomic_store_n(&attr_done[dev], 1, __ATOMIC_RELEASE);
+    }
+    auto launch = [&](auto kernel) {
+        gj_launch_pdl(kernel, dim3(grid), dim3(HD_THREADS), smem, stream, a->d_file, a->d_file + a->file_size, a->d_seg_off,
                       a->seg_count, a->seg_mcu, *a, own, a->d_coef, a->d_cext, a->d_tables);
-    else
-        gj_launch_pdl(k_huff_decode<false>, dim3(grid), dim3(HD_THREADS), 0, stream, a->d_file, a->d_file + a->file_size, a->d_seg_off,
-                      a->seg_count, a->seg_mcu, *a, own, a->d_coef, a->d_cext, a->d_tables);
+    };
+    if ( own.cmp_words ) {
+        if ( a->dequantize ) launch(k_huff_decode<true, true>);
+        else launch(k_huff_decode<false, true>);
+    }
+    else {
+        if ( a->dequantize ) launch(k_huff_decode<true, false>);
+        else launch(k_huff_decode<false, false>);
+    }
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
