@@ -294,8 +294,9 @@ class Encoder:
 class Decoder:
     """gpujpeg_decoder_create / gpujpeg_decoder_decode / gpujpeg_decoder_destroy"""
 
-    def __init__(self, stream=0, idct="int", scale="1"):
-        """scale: "1", "1/2", "1/4" or "1/8" -- decode to ceil(W * scale) x ceil(H * scale) pixels (dec_opt_scale)"""
+    def __init__(self, stream=0, idct="int", scale="1", crop=None):
+        """scale: "1", "1/2", "1/4" or "1/8" -- decode to ceil(W * scale) x ceil(H * scale) pixels (dec_opt_scale)
+        crop: (x, y, w, h) -- return only that rectangle of the (scaled) image (dec_opt_crop)"""
         self._h = lib.gpujpeg_decoder_create(C.c_void_p(stream))
         if not self._h:
             raise GpuJpegError("gpujpeg_decoder_create failed (no CUDA device?)")
@@ -303,6 +304,9 @@ class Decoder:
             self.set_option("dec_opt_idct", idct)
         if scale != "1":
             self.set_option("dec_opt_scale", scale)
+        if crop is not None:
+            x, y, w, h = (int(v) for v in crop)
+            self.set_option("dec_opt_crop", "%dx%d+%d+%d" % (w, h, x, y))
 
     def set_option(self, key, val):
         if lib.gpujpeg_decoder_set_option(self._h, key.encode(), val.encode()) != 0:

@@ -213,6 +213,73 @@ int gj_geometry_init(struct gj_geometry* g, const struct gpujpeg_parameters* par
     return 0;
 }
 
+void gj_crop_blocks(const struct gj_geometry* g, int n, int x, int y, int w, int h, struct gj_blk_rect win[GJ_MAX_COMP])
+{
+    memset(win, 0, sizeof(struct gj_blk_rect) * GJ_MAX_COMP);
+    for ( int c = 0; c < g->comp_count; c++ ) {
+        const int dh = g->max_hs / g->comp[c].hs, dv = g->max_vs / g->comp[c].vs;
+        win[c].bx0 = x / dh / n;
+        win[c].by0 = y / dv / n;
+        win[c].bx1 = (x + w - 1) / dh / n + 1;
+        win[c].by1 = (y + h - 1) / dv / n + 1;
+    }
+}
+
+int gj_crop_pick_units(int units_x, int units, int seg_units, int bpm, int ux0, int uy0, int ux1, int uy1, int seg_base,
+                       uint32_t* out)
+{
+    int n = 0;
+    for ( int uy = uy0; uy < uy1; uy++ ) {
+        /* the row's needed units [u, u_end); a segment may hold pieces of several rows, so merge with the previous entry */
+        int u = uy * units_x + ux0;
+        const int u_end = uy * units_x + (ux1 < units_x ? ux1 : units_x);
+        while ( u < u_end && u < units ) {
+            const int s = u / seg_units;
+            int last = (s + 1) * seg_units;
+            if ( last > u_end ) last = u_end;
+            if ( last > units ) last = units;
+            const uint32_t blocks = (uint32_t)(last - s * seg_units) * (uint32_t)bpm;   /* through unit last - 1 */
+            if ( n > 0 && out[2 * (n - 1)] == (uint32_t)(seg_base + s) ) out[2 * (n - 1) + 1] = blocks;
+            else {
+                out[2 * n] = (uint32_t)(seg_base + s);
+                out[2 * n + 1] = blocks;
+                n++;
+            }
+            u = last;
+        }
+    }
+    return n;
+}
+
+/* the unit (MCU) rectangle of a scan: one block per unit for a single component, hs x vs blocks per component otherwise --
+ * every component's window maps to the same MCUs, as they all come from the same pixels */
+static void crop_units(int ncomp, const int* comp, const int* hs, const int* vs, const struct gj_blk_rect* win, int* ux0, int* uy0,
+                       int* ux1, int* uy1)
+{
+    const struct gj_blk_rect* r = &win[comp[0]];
+    const int h = ncomp == 1 ? 1 : hs[0], v = ncomp == 1 ? 1 : vs[0];
+    *ux0 = r->bx0 / h;
+    *uy0 = r->by0 / v;
+    *ux1 = (r->bx1 - 1) / h + 1;
+    *uy1 = (r->by1 - 1) / v + 1;
+}
+
+int gj_crop_pick(const struct gj_geometry* g, int k, const struct gj_blk_rect win[GJ_MAX_COMP], uint32_t* out)
+{
+    const struct gj_scan_layout* l = &g->lay;
+    int comp[GJ_MAX_COMP] = {k, 0, 0, 0}, hs[GJ_MAX_COMP], vs[GJ_MAX_COMP];
+    const int ncomp = g->interleaved ? g->comp_count : 1;
+    for ( int i = 0; i < GJ_MAX_COMP; i++ ) {
+        if ( g->interleaved ) comp[i] = i;
+        hs[i] = g->comp[comp[i]].hs;
+        vs[i] = g->comp[comp[i]].vs;
+    }
+    const int units_x = g->interleaved ? l->mcu_x : g->comp[k].bcx;
+    int ux0, uy0, ux1, uy1;
+    crop_units(ncomp, comp, hs, vs, win, &ux0, &uy0, &ux1, &uy1);
+    return gj_crop_pick_units(units_x, l->scan_mcus[k], g->seg_mcu, l->bpm, ux0, uy0, ux1, uy1, l->scan_seg_begin[k], out);
+}
+
 /* ------------------------------------------------------------------------------------------- */
 /* writer                                                                                        */
 
@@ -904,4 +971,14 @@ int gj_prog_scan_init(const struct gj_geometry* g, const struct gj_stream* s, in
     out->seg_units = restart_interval > 0 ? restart_interval : out->units;
     out->seg_count = (out->units + out->seg_units - 1) / out->seg_units;
     return 0;
+}
+
+/* Every scan of a component decodes the same units (a refinement continues exactly the blocks the earlier scans of its
+ * band decoded); the end-of-band run of the last needed block may reach further, and the scan stops there. */
+int gj_prog_crop_pick(const struct gj_prog_scan* S, const int comp[GJ_MAX_COMP], const struct gj_blk_rect win[GJ_MAX_COMP],
+                      uint32_t* out)
+{
+    int ux0, uy0, ux1, uy1;
+    crop_units(S->ncomp, comp, S->hs, S->vs, win, &ux0, &uy0, &ux1, &uy1);
+    return gj_crop_pick_units(S->units_x, S->units, S->seg_units, S->bpm, ux0, uy0, ux1, uy1, 0, out);
 }

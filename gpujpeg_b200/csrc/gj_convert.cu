@@ -39,6 +39,7 @@ struct ConvertParams {
     int width, height;
     int cs;                 /* colour space of the raw image (enum gpujpeg_color_space) */
     int cs_internal;        /* colour space of the JPEG's components */
+    int x0, y0;             /* decode, dec_opt_crop: raw pixel (x, y) is image pixel (x0 + x, y0 + y) */
 };
 
 __constant__ int c_to_rgb[5][9] = {{0}, {0}, {298, 0, 409, 298, -100, -208, 298, 516, 0},
@@ -92,20 +93,24 @@ k_convert_in(const uint8_t* __restrict__ raw, uint8_t* __restrict__ planes, cons
             raw[p.off[0] + (size_t)y * p.pitch[0] + (size_t)x * p.xs[0] + p.alpha_off];
 }
 
+/* ORIGIN: a rectangle of the image from (p.x0, p.y0) on; the raw image's chroma grid keeps its phase, as x0 (y0) is even
+ * wherever the pixel format subsamples horizontally (vertically) */
+template <bool ORIGIN>
 __global__ void __launch_bounds__(256)
 k_convert_out(const uint8_t* __restrict__ planes, uint8_t* __restrict__ raw, const __grid_constant__ ConvertParams p)
 {
     const int x = blockIdx.x * 256 + threadIdx.x, y = blockIdx.y;
     if ( x >= p.width ) return;
+    const int ix = ORIGIN ? p.x0 + x : x, iy = ORIGIN ? p.y0 + y : y;   /* the image pixel */
     int c[3] = {0, 128, 128};
     const int colour_comps = p.jpeg_comps < 3 ? p.jpeg_comps : 3;
     for ( int k = 0; k < colour_comps; k++ )
-        c[k] = planes[p.poff[k] + (size_t)(y / p.pdv[k]) * p.ppitch[k] + x / p.pdh[k]];
+        c[k] = planes[p.poff[k] + (size_t)(iy / p.pdv[k]) * p.ppitch[k] + ix / p.pdh[k]];
     if ( p.jpeg_comps >= 3 ) cs_transform(p.cs_internal, p.cs, c);
     raw[p.off[0] + (size_t)y * p.pitch[0] + (size_t)x * p.xs[0]] = (uint8_t)c[0];
     if ( p.alpha_off )   /* the stream's fourth component, opaque without one */
         raw[p.off[0] + (size_t)y * p.pitch[0] + (size_t)x * p.xs[0] + p.alpha_off] =
-            p.jpeg_comps == 4 ? planes[p.poff[3] + (size_t)(y / p.pdv[3]) * p.ppitch[3] + x / p.pdh[3]] : (uint8_t)0xFF;
+            p.jpeg_comps == 4 ? planes[p.poff[3] + (size_t)(iy / p.pdv[3]) * p.ppitch[3] + ix / p.pdh[3]] : (uint8_t)0xFF;
     if ( p.raw_comps == 1 ) return;
     if ( p.uyvy ) {
         const int k = (x & 1) ? 2 : 1;
@@ -210,11 +215,14 @@ extern "C" int gj_launch_convert_in(const uint8_t* d_raw, const struct gj_raw_la
 extern "C" int gj_launch_convert_out(const uint8_t* d_planes, uint8_t* d_raw, const struct gj_raw_layout* raw,
                                      enum gpujpeg_pixel_format fmt, int color_space, int color_space_internal, int width,
                                      int height, const struct gj_comp_geo* comp, int comp_count, int max_hs, int max_vs, int n,
-                                     gj_stream_t stream)
+                                     int x0, int y0, gj_stream_t stream)
 {
     ConvertParams p;
     if ( fill_params(&p, raw, fmt, color_space, color_space_internal, width, height, comp, comp_count, max_hs, max_vs, n) ) return -1;
-    k_convert_out<<<dim3((width + 255) / 256, height), 256, 0, stream>>>(d_planes, d_raw, p);
+    p.x0 = x0;
+    p.y0 = y0;
+    if ( x0 || y0 ) k_convert_out<true><<<dim3((width + 255) / 256, height), 256, 0, stream>>>(d_planes, d_raw, p);
+    else k_convert_out<false><<<dim3((width + 255) / 256, height), 256, 0, stream>>>(d_planes, d_raw, p);
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 

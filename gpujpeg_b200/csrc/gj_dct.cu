@@ -481,6 +481,56 @@ k_fdct_rgb_ss(const uint8_t* __restrict__ raw, int width, int height, size_t pit
 /* =========================================================================================== */
 /* K4                                                                                            */
 
+/* dec_opt_crop (WIN instances of the fused kernels): the grid covers the strips and block (MCU) rows from strip0 / row0 that
+ * the rectangle [x, x + w) x [y, y + h) touches, phase A transforms only the blocks [bx0, bx1) x [by0, by1) of each component,
+ * and phase B writes only the rectangle's pixels, pixel (px, py) at (px - x, py - y) of an image of pitch 3w */
+struct FusedWin {
+    int x, y, w, h;
+    int strip0, row0;
+    int bx0[3], bx1[3], by0[3], by1[3];
+};
+
+/* Phase B of a WIN instance.  Groups of 4 output pixels are counted from the rectangle's left edge, so that a group whose 4
+ * pixels lie in this strip and whose destination is 4-byte aligned is stored as three words (every group of a row whose
+ * offset (py - y) * 3w is a multiple of 4); the groups cut by the strip's or the rectangle's edges, and the rows of other
+ * alignment, byte by byte.  fetch(row, lx, Y, Cb, Cr): the samples of strip pixel lx of strip row `row`. */
+template <int ROWS, class Fetch>
+__device__ __forceinline__ void win_phase_b(const FusedWin& w, int x0, int y0, int vw, int vh, int nthreads, uint8_t* __restrict__ raw,
+                                            size_t pitch, Fetch fetch)
+{
+    const int xs = max(x0, w.x), xe = min(x0 + vw, w.x + w.w);
+    if ( xs >= xe ) return;
+    const int ka = (xs - w.x) >> 2, ng = ((xe - 1 - w.x) >> 2) - ka + 1;
+    for ( int g = threadIdx.x; g < ROWS * ng; g += nthreads ) {
+        const int row = g / ng, k = ka + g - row * ng;
+        const int py = y0 + row;
+        if ( row >= vh || py < w.y || py >= w.y + w.h ) continue;
+        const int first = w.x + 4 * k;
+        int r[4], gg[4], bb[4];
+#pragma unroll
+        for ( int j = 0; j < 4; j++ ) {
+            const int lx = min(max(first + j, xs), xe - 1) - x0;   // (pixels outside the rectangle: any valid sample, not stored)
+            int cy, cb, cr;
+            fetch(row, lx, cy, cb, cr);
+            gj_ycbcr_to_rgb_raw(cy, cb, cr, r[j], gg[j], bb[j]);
+        }
+        const uint32_t o[3] = {pack4_sat_u8(r[0], gg[0], bb[0], r[1]), pack4_sat_u8(gg[1], bb[1], r[2], gg[2]),
+                               pack4_sat_u8(bb[2], r[3], gg[3], bb[3])};
+        uint8_t* p = raw + (size_t)(py - w.y) * pitch + (size_t)k * 12;
+        if ( first >= xs && first + 4 <= xe && (reinterpret_cast<uintptr_t>(p) & 3) == 0 ) {
+            uint32_t* q = reinterpret_cast<uint32_t*>(p);
+            q[0] = o[0];
+            q[1] = o[1];
+            q[2] = o[2];
+        }
+        else {
+#pragma unroll
+            for ( int i = 0; i < 12; i++ )
+                if ( first + i / 3 >= xs && first + i / 3 < xe ) p[i] = (uint8_t)(o[i >> 2] >> (8 * (i & 3)));
+        }
+    }
+}
+
 /* integer path == gpujpeg_idct_cpu: dequantised int16 coefficients, rows, columns, +128, clamp
  * [ref: src/gpujpeg_dct_cpu.c:178-189, 239-251].  NZ: how many leading zig-zag coefficients may be non-zero -- 64, or 16
  * for a warp whose blocks all have extent <= 2 (natural rows 0-4, columns 0-5): the others then enter as literal zeros
@@ -504,16 +554,16 @@ __device__ __forceinline__ void idct_int_px(const uint32_t (&packed)[32], const 
 // FLAVOUR 0 = integer IDCT (gpujpeg_idct_cpu), 1 = float GPU-reference IDCT
 // DEQ     true  = coefficients are raw quantised values: multiply by the table here
 //         false = K3 already stored coefficient*quantiser wrapped to int16 (FLAVOUR 0 only)
-template <int VEC, int FLAVOUR, bool DEQ>
+template <int VEC, int FLAVOUR, bool DEQ, bool WIN>
 __global__ void __launch_bounds__(NT)
 k_idct_rgb444(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext, int bcx, int nblk, uint8_t* __restrict__ raw, int width, int height,
-              size_t pitch, const __grid_constant__ IdctParams prm)
+              size_t pitch, const __grid_constant__ IdctParams prm, const __grid_constant__ FusedWin w)
 {
     gj_pdl_wait();
     __shared__ __align__(16) uint8_t s_pl[3 * K4_PLANE];
 
-    const int bx0 = blockIdx.x * TB;
-    const int by = blockIdx.y;
+    const int bx0 = (WIN ? w.strip0 + (int)blockIdx.x : (int)blockIdx.x) * TB;
+    const int by = WIN ? w.row0 + (int)blockIdx.y : (int)blockIdx.y;
     const int x0 = bx0 * 8;
     const int vw = min(STRIP_PX, width - x0);
     const int vh = min(8, height - by * 8);
@@ -522,7 +572,7 @@ k_idct_rgb444(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
     {
         const int comp = threadIdx.x >> 6;
         const int b = threadIdx.x & 63;
-        const bool in = bx0 + b < bcx;
+        const bool in = bx0 + b < bcx && (!WIN || (bx0 + b >= w.bx0[comp] && bx0 + b < w.bx1[comp]));
         const size_t bi = (size_t)comp * nblk + (size_t)by * bcx + bx0 + b;
         const int ext = in ? __ldg(cext + bi) : 0;
         const bool head = __all_sync(0xFFFFFFFFu, ext <= 2);   // warp-uniform: a warp holds blocks of one component
@@ -559,6 +609,14 @@ k_idct_rgb444(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
     }
     __syncthreads();
 
+    if constexpr ( WIN ) {
+        win_phase_b<8>(w, x0, by * 8, vw, vh, NT, raw, pitch, [&](int row, int lx, int& cy, int& cb, int& cr) {
+            cy = s_pl[row * STRIP_PX + lx];
+            cb = s_pl[K4_PLANE + row * STRIP_PX + lx];
+            cr = s_pl[2 * K4_PLANE + row * STRIP_PX + lx];
+        });
+        return;
+    }
     /* phase B: 4 pixels per step: 3 plane words -> 3 interleaved words, straight to global memory */
     uint8_t* out = raw + (size_t)by * 8 * pitch + (size_t)x0 * 3;
     for ( int g = threadIdx.x; g < GROUPS; g += NT ) {
@@ -594,10 +652,10 @@ k_idct_rgb444(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
 
 /* K4 with chroma subsampling: the mirror image of k_fdct_rgb_ss.  Every pixel takes the chrominance sample at
  * (x / HS, y / VS) -- sample replication, as the reference's postprocessor [ref: src/gpujpeg_postprocessor.cu:55-76]. */
-template <int HS, int VS, int VEC, int FLAVOUR, bool DEQ>
+template <int HS, int VS, int VEC, int FLAVOUR, bool DEQ, bool WIN>
 __global__ void __launch_bounds__(TB * VS + 2 * TB / HS)
 k_idct_rgb_ss(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext, const __grid_constant__ SsGrid grid, uint8_t* __restrict__ raw, int width,
-              int height, size_t pitch, const __grid_constant__ IdctParams prm)
+              int height, size_t pitch, const __grid_constant__ IdctParams prm, const __grid_constant__ FusedWin w)
 {
     gj_pdl_wait();
     constexpr int NTS = TB * VS + 2 * TB / HS;
@@ -606,9 +664,10 @@ k_idct_rgb_ss(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
     __shared__ __align__(16) uint8_t s_y[8 * VS * STRIP_PX];
     __shared__ __align__(16) uint8_t s_c[2][8 * CW];
 
-    const int bx0 = blockIdx.x * TB;
+    const int sx = WIN ? w.strip0 + (int)blockIdx.x : (int)blockIdx.x, sy = WIN ? w.row0 + (int)blockIdx.y : (int)blockIdx.y;
+    const int bx0 = sx * TB;
     const int x0 = bx0 * 8;
-    const int y0 = blockIdx.y * 8 * VS;
+    const int y0 = sy * 8 * VS;
     const int vw = min(STRIP_PX, width - x0);
     const int vh = min(8 * VS, height - y0);
 
@@ -620,7 +679,7 @@ k_idct_rgb_ss(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
             comp = 0;
             const int b = threadIdx.x & (TB - 1), byl = threadIdx.x / TB;
             bx = bx0 + b;
-            by = blockIdx.y * VS + byl;
+            by = sy * VS + byl;
             dst = s_y + byl * 8 * STRIP_PX + b * 8;
             dpitch = STRIP_PX;
         }
@@ -628,11 +687,12 @@ k_idct_rgb_ss(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
             const int u = threadIdx.x - TB * VS;
             comp = 1 + u / CB;
             bx = bx0 / HS + u % CB;
-            by = blockIdx.y;
+            by = sy;
             dst = s_c[comp - 1] + (u % CB) * 8;
             dpitch = CW;
         }
-        const bool in = bx < grid.bcx[comp] && by < grid.bcy[comp];
+        const bool in = bx < grid.bcx[comp] && by < grid.bcy[comp] &&
+                        (!WIN || (bx >= w.bx0[comp] && bx < w.bx1[comp] && by >= w.by0[comp] && by < w.by1[comp]));
         const size_t bi = (size_t)grid.blk_off[comp] + (size_t)by * grid.bcx[comp] + bx;
         const int ext = in ? __ldg(cext + bi) : 0;
         const bool head = __all_sync(0xFFFFFFFFu, ext <= 2);   // warp-uniform: a warp holds blocks of one component
@@ -665,6 +725,14 @@ k_idct_rgb_ss(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
     }
     __syncthreads();
 
+    if constexpr ( WIN ) {
+        win_phase_b<8 * VS>(w, x0, y0, vw, vh, NTS, raw, pitch, [&](int row, int lx, int& cy, int& cb, int& cr) {
+            cy = s_y[row * STRIP_PX + lx];
+            cb = s_c[0][(row / VS) * CW + lx / HS];
+            cr = s_c[1][(row / VS) * CW + lx / HS];
+        });
+        return;
+    }
     uint8_t* out = raw + (size_t)y0 * pitch + (size_t)x0 * 3;
     for ( int g = threadIdx.x; g < GROUPS * VS; g += NTS ) {
         const int row = g >> 7, gx = g & 127;
@@ -717,6 +785,36 @@ struct SampleGrid {
 };
 constexpr int SG_THREADS = 128;
 
+/* dec_opt_crop (WIN instances): thread i takes window block i -- component c's blocks [bx0, bx0 + wbx) x [by0, ..) are window
+ * blocks [first[c], first[c + 1]) in raster order --, and sample (sx, sy) of component c goes to (sx - ox, sy - oy), kept
+ * inside g.cw x g.ch */
+struct BlockWin {
+    int bx0[GJ_MAX_COMP], by0[GJ_MAX_COMP], wbx[GJ_MAX_COMP], ox[GJ_MAX_COMP], oy[GJ_MAX_COMP], first[GJ_MAX_COMP + 1];
+};
+/* window thread -> component, block column / row and block index */
+__device__ __forceinline__ int win_block(const BlockWin& w, const SampleGrid& g, int wi, int& comp, int& bx, int& by)
+{
+    comp = (wi >= w.first[1]) + (wi >= w.first[2]) + (wi >= w.first[3]);
+    const int local = wi - w.first[comp];
+    const int wy = local / w.wbx[comp];
+    bx = w.bx0[comp] + local - wy * w.wbx[comp];
+    by = w.by0[comp] + wy;
+    return g.blk_off[comp] + by * g.bcx[comp] + bx;
+}
+/* the N x N samples of a block whose first sample lands at (x0, y0) of the raw image: only those inside cw x ch, byte by byte */
+template <int N, class Get>
+__device__ __forceinline__ void win_store(uint8_t* raw, const SampleGrid& g, int comp, int x0, int y0, Get px)
+{
+#pragma unroll
+    for ( int y = 0; y < N; y++ ) {
+        if ( y0 + y < 0 || y0 + y >= g.ch[comp] ) continue;
+#pragma unroll
+        for ( int x = 0; x < N; x++ )
+            if ( x0 + x >= 0 && x0 + x < g.cw[comp] )
+                raw[g.off[comp] + (long long)(y0 + y) * (long long)g.pitch[comp] + (long long)(x0 + x) * g.xs[comp]] = px(x, y);
+    }
+}
+
 __global__ void __launch_bounds__(SG_THREADS)
 k_fdct_samples(const uint8_t* __restrict__ raw, const __grid_constant__ SampleGrid g, int total_blocks,
                int16_t* __restrict__ coef, uint64_t* __restrict__ nzmask, const __grid_constant__ FdctParams prm)
@@ -748,18 +846,25 @@ k_fdct_samples(const uint8_t* __restrict__ raw, const __grid_constant__ SampleGr
     quantise_store(v, prm.fwd_zz[g.table[comp]], coef + (size_t)bi * 64, nzmask + bi);
 }
 
-template <int FLAVOUR, bool DEQ>
+template <int FLAVOUR, bool DEQ, bool WIN>
 __global__ void __launch_bounds__(SG_THREADS)
 k_idct_samples(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext, const __grid_constant__ SampleGrid g, int total_blocks,
-               uint8_t* __restrict__ raw, const __grid_constant__ IdctParams prm)
+               uint8_t* __restrict__ raw, const __grid_constant__ IdctParams prm, const __grid_constant__ BlockWin w)
 {
-    const int bi = blockIdx.x * SG_THREADS + threadIdx.x;
+    int bi = blockIdx.x * SG_THREADS + threadIdx.x;
     if ( bi >= total_blocks ) return;
-    const int comp = (bi >= g.blk_off[1]) + (bi >= g.blk_off[2]) + (bi >= g.blk_off[3]);
-    const int local = bi - g.blk_off[comp];
-    const int by = local / g.bcx[comp], bx = local - by * g.bcx[comp];
-    const int vw = min(8, g.cw[comp] - bx * 8), vh = min(8, g.ch[comp] - by * 8);
-    if ( vw <= 0 || vh <= 0 ) return;
+    int comp, by, bx;
+    if constexpr ( WIN ) {
+        bi = win_block(w, g, bi, comp, bx, by);
+    }
+    else {
+        comp = (bi >= g.blk_off[1]) + (bi >= g.blk_off[2]) + (bi >= g.blk_off[3]);
+        const int local = bi - g.blk_off[comp];
+        by = local / g.bcx[comp];
+        bx = local - by * g.bcx[comp];
+    }
+    int vw = min(8, g.cw[comp] - bx * 8), vh = min(8, g.ch[comp] - by * 8);
+    if ( !WIN && (vw <= 0 || vh <= 0) ) return;
     uint32_t packed[32];
     gj_load_coef_block(coef + (size_t)bi * 64, __ldg(cext + bi), packed);
     const uint16_t* q = prm.q_zz[comp];
@@ -789,7 +894,20 @@ k_idct_samples(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cex
             px[i] = pack4_sat_u8(GJ_RINT(GJ_FADD(f[4 * i], 128.0f)), GJ_RINT(GJ_FADD(f[4 * i + 1], 128.0f)),
                                  GJ_RINT(GJ_FADD(f[4 * i + 2], 128.0f)), GJ_RINT(GJ_FADD(f[4 * i + 3], 128.0f)));
     }
-    uint8_t* dst = raw + g.off[comp] + (size_t)by * 8 * g.pitch[comp] + (size_t)bx * 8 * g.xs[comp];
+    uint8_t* dst;
+    if constexpr ( WIN ) {
+        /* a block on the window's edge byte by byte; an interior one as below, with whole-row stores where aligned */
+        const int x0 = bx * 8 - w.ox[comp], y0 = by * 8 - w.oy[comp];
+        if ( x0 < 0 || y0 < 0 || x0 + 8 > g.cw[comp] || y0 + 8 > g.ch[comp] ) {
+            win_store<8>(raw, g, comp, x0, y0, [&](int x, int y) { return (uint8_t)(px[2 * y + (x >> 2)] >> (8 * (x & 3))); });
+            return;
+        }
+        dst = raw + g.off[comp] + (size_t)y0 * g.pitch[comp] + (size_t)x0 * g.xs[comp];
+        vw = vh = 8;
+    }
+    else {
+        dst = raw + g.off[comp] + (size_t)by * 8 * g.pitch[comp] + (size_t)bx * 8 * g.xs[comp];
+    }
     const bool rows8 = g.xs[comp] == 1 && vw == 8 && ((reinterpret_cast<uintptr_t>(dst) | g.pitch[comp]) & 7) == 0;
 #pragma unroll
     for ( int y = 0; y < 8; y++ ) {
@@ -808,18 +926,25 @@ k_idct_samples(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cex
 /* Scaled decoding (dec_opt_scale): libjpeg's reduced IDCT (gj_idct_scaled_block), N x N samples per block, one thread per
  * block as k_idct_samples.  The coefficients are the raw quantised values; they are dequantised here in 32 bits.  Only the
  * chunks below the block's extent are loaded (at N = 1 only the DC); g.cw / g.ch count samples of the scaled component. */
-template <int N>
+template <int N, bool WIN>
 __global__ void __launch_bounds__(SG_THREADS)
 k_idct_scaled(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext, const __grid_constant__ SampleGrid g, int total_blocks,
-              uint8_t* __restrict__ raw, const __grid_constant__ IdctParams prm)
+              uint8_t* __restrict__ raw, const __grid_constant__ IdctParams prm, const __grid_constant__ BlockWin w)
 {
-    const int bi = blockIdx.x * SG_THREADS + threadIdx.x;
+    int bi = blockIdx.x * SG_THREADS + threadIdx.x;
     if ( bi >= total_blocks ) return;
-    const int comp = (bi >= g.blk_off[1]) + (bi >= g.blk_off[2]) + (bi >= g.blk_off[3]);
-    const int local = bi - g.blk_off[comp];
-    const int by = local / g.bcx[comp], bx = local - by * g.bcx[comp];
+    int comp, by, bx;
+    if constexpr ( WIN ) {
+        bi = win_block(w, g, bi, comp, bx, by);
+    }
+    else {
+        comp = (bi >= g.blk_off[1]) + (bi >= g.blk_off[2]) + (bi >= g.blk_off[3]);
+        const int local = bi - g.blk_off[comp];
+        by = local / g.bcx[comp];
+        bx = local - by * g.bcx[comp];
+    }
     const int vw = min(N, g.cw[comp] - bx * N), vh = min(N, g.ch[comp] - by * N);
-    if ( vw <= 0 || vh <= 0 ) return;
+    if ( !WIN && (vw <= 0 || vh <= 0) ) return;
     const uint16_t* q = prm.q_zz[comp];
     const int ext = __ldg(cext + bi);
     int v[64];
@@ -837,6 +962,10 @@ k_idct_scaled(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
     }
     int px[N * N];
     gj_idct_scaled_block<N>(v, px);
+    if constexpr ( WIN ) {
+        win_store<N>(raw, g, comp, bx * N - w.ox[comp], by * N - w.oy[comp], [&](int x, int y) { return (uint8_t)px[N * y + x]; });
+        return;
+    }
     uint8_t* dst = raw + g.off[comp] + (size_t)by * N * g.pitch[comp] + (size_t)bx * N * g.xs[comp];
 #pragma unroll
     for ( int y = 0; y < N; y++ ) {
@@ -929,7 +1058,8 @@ static int launch_idct_rgb444(const int16_t* d_coef, const uint8_t* d_cext, int 
     const dim3 grid((bcx + TB - 1) / TB, bcy);
     const int vec = pick_vec(d_raw, (size_t)pitch);
     if ( idct_flavour != 0 && coef_dequantized ) return -1;   // the float flavour needs raw coefficients
-#define GJ_K4(V, F, D) gj_launch_pdl(k_idct_rgb444<V, F, D>, grid, dim3(NT), 0, stream, d_coef, d_cext, bcx, nblk, d_raw, width, height, (size_t)pitch, prm)
+    const FusedWin nowin = {};
+#define GJ_K4(V, F, D) gj_launch_pdl(k_idct_rgb444<V, F, D, false>, grid, dim3(NT), 0, stream, d_coef, d_cext, bcx, nblk, d_raw, width, height, (size_t)pitch, prm, nowin)
     if ( idct_flavour == 0 && coef_dequantized ) {
         if ( vec == 4 ) GJ_K4(4, 0, false); else GJ_K4(1, 0, false);
     }
@@ -1044,8 +1174,9 @@ extern "C" int gj_launch_idct_rgb_ss_rows(const int16_t* d_coef, const uint8_t* 
     d_raw += (ptrdiff_t)my0 * 8 * vs * pitch;
     const dim3 grid((comp[0].bcx + TB - 1) / TB, my1 - my0);
     const int vec = pick_vec(d_raw, (size_t)pitch);
+    const FusedWin nowin = {};
 #define GJ_K4SS2(H, V, VE, F, D) \
-    gj_launch_pdl(k_idct_rgb_ss<H, V, VE, F, D>, grid, dim3(TB * V + 2 * TB / H), 0, stream, d_coef, d_cext, sg, d_raw, width, height, (size_t)pitch, prm)
+    gj_launch_pdl(k_idct_rgb_ss<H, V, VE, F, D, false>, grid, dim3(TB * V + 2 * TB / H), 0, stream, d_coef, d_cext, sg, d_raw, width, height, (size_t)pitch, prm, nowin)
 #define GJ_K4SS(H, V)                                                                  \
     do {                                                                               \
         if ( idct_flavour == 0 && coef_dequantized ) {                                 \
@@ -1073,6 +1204,63 @@ extern "C" int gj_launch_idct_rgb_ss(const int16_t* d_coef, const uint8_t* d_cex
     const int vs = comp[0].vs > 0 ? comp[0].vs : 1;
     return gj_launch_idct_rgb_ss_rows(d_coef, d_cext, comp, 0, (comp[0].bcy + vs - 1) / vs, comp_tq, d_raw, width, height, pitch,
                                       idct_flavour, coef_dequantized, h_tables, stream);
+}
+
+/* dec_opt_crop on the fused kernels: the rectangle [x, x + w) x [y, y + h) of the RGB image into d_out (pitch 3w); 4:4:4 when
+ * every component is 1x1, else the chroma-subsampling instance */
+extern "C" int gj_launch_idct_rgb_window(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], const int comp_tq[3],
+                                         uint8_t* d_out, int width, int height, int x, int y, int w, int h, int idct_flavour,
+                                         int coef_dequantized, const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
+{
+    IdctParams prm;
+    for ( int c = 0; c < 3; c++ )
+        memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c]], sizeof prm.q_zz[c]);
+    if ( idct_flavour != 0 && coef_dequantized ) return -1;
+    if ( w < 1 || h < 1 || x < 0 || y < 0 || x + w > width || y + h > height ) return -1;
+    const int hs = comp[0].hs, vs = comp[0].vs;
+    if ( comp[1].hs != 1 || comp[1].vs != 1 || comp[2].hs != 1 || comp[2].vs != 1 ) return -1;
+    FusedWin fw;
+    memset(&fw, 0, sizeof fw);
+    fw.x = x;
+    fw.y = y;
+    fw.w = w;
+    fw.h = h;
+    fw.strip0 = x / STRIP_PX;
+    fw.row0 = y / (8 * vs);
+    for ( int c = 0; c < 3; c++ ) {
+        const int dh = hs / comp[c].hs, dv = vs / comp[c].vs;
+        fw.bx0[c] = x / dh / 8;
+        fw.bx1[c] = (x + w - 1) / dh / 8 + 1;
+        fw.by0[c] = y / dv / 8;
+        fw.by1[c] = (y + h - 1) / dv / 8 + 1;
+    }
+    const dim3 grid((x + w - 1) / STRIP_PX - fw.strip0 + 1, (y + h - 1) / (8 * vs) - fw.row0 + 1);
+    const size_t pitch = (size_t)w * 3;
+    if ( hs == 1 && vs == 1 ) {
+#define GJ_K4W(F, D) gj_launch_pdl(k_idct_rgb444<4, F, D, true>, grid, dim3(NT), 0, stream, d_coef, d_cext, comp[0].bcx, comp[0].nblk, d_out, width, height, pitch, prm, fw)
+        if ( idct_flavour == 0 && coef_dequantized ) GJ_K4W(0, false);
+        else if ( idct_flavour == 0 ) GJ_K4W(0, true);
+        else GJ_K4W(1, true);
+#undef GJ_K4W
+        return cudaGetLastError() == cudaSuccess ? 0 : -1;
+    }
+    SsGrid sg;
+    ss_grid_rows(&sg, comp, 0, (comp[0].bcy + vs - 1) / vs, height);
+#define GJ_K4WS2(H, V, F, D) \
+    gj_launch_pdl(k_idct_rgb_ss<H, V, 4, F, D, true>, grid, dim3(TB * V + 2 * TB / H), 0, stream, d_coef, d_cext, sg, d_out, width, height, pitch, prm, fw)
+#define GJ_K4WS(H, V)                                                          \
+    do {                                                                       \
+        if ( idct_flavour == 0 && coef_dequantized ) GJ_K4WS2(H, V, 0, false); \
+        else if ( idct_flavour == 0 ) GJ_K4WS2(H, V, 0, true);                 \
+        else GJ_K4WS2(H, V, 1, true);                                          \
+    } while ( 0 )
+    if ( hs == 2 && vs == 2 ) GJ_K4WS(2, 2);
+    else if ( hs == 2 && vs == 1 ) GJ_K4WS(2, 1);
+    else if ( hs == 1 && vs == 2 ) GJ_K4WS(1, 2);
+    else return -1;
+#undef GJ_K4WS
+#undef GJ_K4WS2
+    return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
 /* ---- no colour transform: grey, planar and packed YCbCr formats ---- */
@@ -1114,41 +1302,76 @@ extern "C" int gj_launch_fdct_samples(const uint8_t* d_raw, const struct gj_raw_
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
+/* the window of gj_k4_window as the WIN kernels take it; returns the number of window blocks */
+static int block_win(BlockWin* bw, const struct gj_k4_window* win, int comp_count)
+{
+    memset(bw, 0, sizeof *bw);
+    int total = 0;
+    for ( int c = 0; c < GJ_MAX_COMP; c++ ) {
+        bw->first[c] = c < comp_count ? total : 0x7FFFFFFF;
+        if ( c >= comp_count ) continue;
+        const struct gj_blk_rect* r = &win->blk[c];
+        bw->bx0[c] = r->bx0;
+        bw->by0[c] = r->by0;
+        bw->wbx[c] = r->bx1 > r->bx0 ? r->bx1 - r->bx0 : 1;
+        bw->ox[c] = win->ox[c];
+        bw->oy[c] = win->oy[c];
+        if ( r->bx1 > r->bx0 && r->by1 > r->by0 ) total += (r->bx1 - r->bx0) * (r->by1 - r->by0);
+    }
+    bw->first[GJ_MAX_COMP] = 0x7FFFFFFF;
+    return total;
+}
+
 extern "C" int gj_launch_idct_samples(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
                                       const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int idct_flavour, int coef_dequantized,
-                                      const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
+                                      const struct gj_dev_dec_tables* h_tables, const struct gj_k4_window* win, gj_stream_t stream)
 {
     IdctParams prm;
     for ( int c = 0; c < GJ_MAX_COMP; c++ )
         memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c < comp_count ? c : 0]], sizeof prm.q_zz[c]);
     SampleGrid sg;
-    const int total = sample_grid(&sg, raw, comp, comp_count, nullptr);
+    int total = sample_grid(&sg, raw, comp, comp_count, nullptr);
     if ( total <= 0 ) return -1;
     if ( idct_flavour != 0 && coef_dequantized ) return -1;
+    BlockWin bw;
+    memset(&bw, 0, sizeof bw);
+    if ( win && (total = block_win(&bw, win, comp_count)) <= 0 ) return -1;
     const int grid = (total + SG_THREADS - 1) / SG_THREADS;
-    if ( idct_flavour == 0 && coef_dequantized )
-        k_idct_samples<0, false><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
-    else if ( idct_flavour == 0 )
-        k_idct_samples<0, true><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
-    else
-        k_idct_samples<1, true><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
+#define GJ_K4S(F, D)                                                                                                                 \
+    do {                                                                                                                             \
+        if ( win ) k_idct_samples<F, D, true><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);          \
+        else k_idct_samples<F, D, false><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);               \
+    } while ( 0 )
+    if ( idct_flavour == 0 && coef_dequantized ) GJ_K4S(0, false);
+    else if ( idct_flavour == 0 ) GJ_K4S(0, true);
+    else GJ_K4S(1, true);
+#undef GJ_K4S
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
 extern "C" int gj_launch_idct_scaled(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
                                      const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int n,
-                                     const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
+                                     const struct gj_dev_dec_tables* h_tables, const struct gj_k4_window* win, gj_stream_t stream)
 {
     IdctParams prm;
     for ( int c = 0; c < GJ_MAX_COMP; c++ )
         memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c < comp_count ? c : 0]], sizeof prm.q_zz[c]);
     SampleGrid sg;
-    const int total = sample_grid(&sg, raw, comp, comp_count, nullptr);
+    int total = sample_grid(&sg, raw, comp, comp_count, nullptr);
     if ( total <= 0 ) return -1;
+    BlockWin bw;
+    memset(&bw, 0, sizeof bw);
+    if ( win && (total = block_win(&bw, win, comp_count)) <= 0 ) return -1;
     const int grid = (total + SG_THREADS - 1) / SG_THREADS;
-    if ( n == 4 ) k_idct_scaled<4><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
-    else if ( n == 2 ) k_idct_scaled<2><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
-    else if ( n == 1 ) k_idct_scaled<1><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm);
+#define GJ_K4R(N)                                                                                                                    \
+    do {                                                                                                                             \
+        if ( win ) k_idct_scaled<N, true><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);              \
+        else k_idct_scaled<N, false><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);                   \
+    } while ( 0 )
+    if ( n == 4 ) GJ_K4R(4);
+    else if ( n == 2 ) GJ_K4R(2);
+    else if ( n == 1 ) GJ_K4R(1);
     else return -1;
+#undef GJ_K4R
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

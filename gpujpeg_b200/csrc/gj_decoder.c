@@ -67,6 +67,16 @@ struct gpujpeg_decoder {
     int out_w, out_h;
     size_t out_size;
     struct gj_comp_geo scomp[GJ_MAX_COMP];
+    /* dec_opt_crop: crop_req = the option is set, crop_r* its rectangle in output pixels; crop = the frame being / last decoded
+     * is cropped, crop_x / _y / _w / _h its rectangle (kept apart from the option, as scale from scale_req, so that a resident
+     * re-run always works on the frame's own rectangle),
+     * crop_blk the blocks of every component it needs, d_pick / h_pick the segments K3 (or every progressive
+     * scan) decodes: {segment, blocks} pairs */
+    int crop_req, crop_rx, crop_ry, crop_rw, crop_rh;
+    int crop, crop_x, crop_y, crop_w, crop_h;
+    struct gj_blk_rect crop_blk[GJ_MAX_COMP];
+    uint32_t* d_pick; size_t d_pick_size;
+    uint32_t* h_pick; size_t h_pick_size;
     struct gpujpeg_image_metadata metadata;
 
     struct gj_dev_dec_tables h_tab, h_tab_prev;
@@ -202,6 +212,8 @@ int gpujpeg_decoder_destroy(struct gpujpeg_decoder* d)
     gj_cuda_free(d->d_raw);
     gj_cuda_free_host(d->h_raw);
     gj_cuda_free(d->d_prog_luts);
+    gj_cuda_free(d->d_pick);
+    free(d->h_pick);
     free(d->prog_scans);
     free(d->h_prog_luts);
     if ( d->copy_stream ) gj_cuda_stream_destroy(d->copy_stream);
@@ -373,36 +385,74 @@ static int launch_k4_scaled(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_
     const struct gj_geometry* g = &d->geo;
     const int n = 8 / d->scale;
     if ( d->out_mode == GJ_OUT_SAMPLES )
-        return gj_launch_idct_scaled(d->d_coef, d->d_cext, d->scomp, g->comp_count, comp_tq, d_out, &d->raw, n, &d->h_tab, d->stream);
+        return gj_launch_idct_scaled(d->d_coef, d->d_cext, d->scomp, g->comp_count, comp_tq, d_out, &d->raw, n, &d->h_tab, NULL, d->stream);
     struct gj_raw_layout pl;
     struct gj_comp_geo padded[GJ_MAX_COMP];
     gj_planes_layout(&pl, padded, g->comp, g->comp_count, n);
-    if ( gj_launch_idct_scaled(d->d_coef, d->d_cext, padded, g->comp_count, comp_tq, d->d_planes, &pl, n, &d->h_tab, d->stream) )
+    if ( gj_launch_idct_scaled(d->d_coef, d->d_cext, padded, g->comp_count, comp_tq, d->d_planes, &pl, n, &d->h_tab, NULL, d->stream) )
         return -1;
     return gj_launch_convert_out(d->d_planes, d_out, &d->raw, d->param_image.pixel_format, d->param_image.color_space,
                                  d->param.color_space_internal, d->out_w, d->out_h, g->comp, g->comp_count, g->max_hs, g->max_vs, n,
-                                 d->stream);
+                                 0, 0, d->stream);
+}
+
+/* K4 of a cropped frame: the blocks of the rectangle only -- RGB through the window instances of the fused kernels, the stream's
+ * own samples straight into the output (GJ_OUT_SAMPLES: component c's sample at the rectangle's origin lands on the output's
+ * (0, 0)), anything else through the component planes and the generic pass over the rectangle's pixels */
+static int launch_k4_crop(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], uint8_t* d_out, int coef_dequantized)
+{
+    const struct gj_geometry* g = &d->geo;
+    const int n = 8 / d->scale;
+    struct gj_k4_window win;
+    memset(&win, 0, sizeof win);
+    memcpy(win.blk, d->crop_blk, sizeof win.blk);
+    struct gj_raw_layout pl;
+    struct gj_comp_geo padded[GJ_MAX_COMP];
+    if ( d->out_mode == GJ_OUT_RGB )   /* the fused kernels' window instances */
+        return gj_launch_idct_rgb_window(d->d_coef, d->d_cext, g->comp, comp_tq, d_out, g->width, g->height, d->crop_x, d->crop_y, d->crop_w,
+                                         d->crop_h, d->idct_flavour, coef_dequantized, &d->h_tab, d->stream);
+    const int direct = d->out_mode == GJ_OUT_SAMPLES;
+    if ( direct ) {
+        for ( int c = 0; c < g->comp_count; c++ ) {
+            win.ox[c] = d->crop_x / (g->max_hs / g->comp[c].hs);
+            win.oy[c] = d->crop_y / (g->max_vs / g->comp[c].vs);
+        }
+    }
+    else {
+        gj_planes_layout(&pl, padded, g->comp, g->comp_count, n);
+    }
+    const struct gj_comp_geo* comp = direct ? d->scomp : padded;
+    uint8_t* dst = direct ? d_out : d->d_planes;
+    const struct gj_raw_layout* rl = direct ? &d->raw : &pl;
+    const int rc = d->scale > 1 ? gj_launch_idct_scaled(d->d_coef, d->d_cext, comp, g->comp_count, comp_tq, dst, rl, n, &d->h_tab, &win, d->stream)
+                                : gj_launch_idct_samples(d->d_coef, d->d_cext, comp, g->comp_count, comp_tq, dst, rl, d->idct_flavour,
+                                                         coef_dequantized, &d->h_tab, &win, d->stream);
+    if ( rc || direct ) return rc;
+    return gj_launch_convert_out(d->d_planes, d_out, &d->raw, d->param_image.pixel_format, d->param_image.color_space,
+                                 d->param.color_space_internal, d->out_w, d->out_h, g->comp, g->comp_count, g->max_hs, g->max_vs, n,
+                                 d->crop_x, d->crop_y, d->stream);
 }
 
 /* K4 for the coder's geometry: the 4:4:4 kernel or the chroma-subsampling template instance */
 static int launch_k4(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], uint8_t* d_out, int coef_dequantized)
 {
     const struct gj_geometry* g = &d->geo;
+    if ( d->crop ) return launch_k4_crop(d, comp_tq, d_out, coef_dequantized);
     if ( d->scale > 1 ) return launch_k4_scaled(d, comp_tq, d_out);
     if ( d->out_mode == GJ_OUT_SAMPLES )
         return gj_launch_idct_samples(d->d_coef, d->d_cext, g->comp, g->comp_count, comp_tq, d_out, &d->raw, d->idct_flavour,
-                                      coef_dequantized, &d->h_tab, d->stream);
+                                      coef_dequantized, &d->h_tab, NULL, d->stream);
     if ( d->out_mode == GJ_OUT_GENERIC ) {
         struct gj_raw_layout pl;
         struct gj_comp_geo padded[GJ_MAX_COMP];
         gj_planes_layout(&pl, padded, g->comp, g->comp_count, 8);
         if ( gj_launch_idct_samples(d->d_coef, d->d_cext, padded, g->comp_count, comp_tq, d->d_planes, &pl, d->idct_flavour,
-                                    coef_dequantized, &d->h_tab, d->stream) )
+                                    coef_dequantized, &d->h_tab, NULL, d->stream) )
             return -1;
         if ( d->flipped && gj_launch_flip_planes(d->d_planes, padded, g->comp_count, d->stream) ) return -1;
         return gj_launch_convert_out(d->d_planes, d_out, &d->raw, d->param_image.pixel_format, d->param_image.color_space,
                                      d->param.color_space_internal,
-                                     g->width, g->height, g->comp, g->comp_count, g->max_hs, g->max_vs, 8, d->stream);
+                                     g->width, g->height, g->comp, g->comp_count, g->max_hs, g->max_vs, 8, 0, 0, d->stream);
     }
     /* dec_opt_flipped on the fused path (see gpujpeg_decoder_decode): rows are written last to first */
     int pitch = g->pitch;
@@ -422,7 +472,7 @@ static int launch_k4(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], 
 static int stripes_usable(struct gpujpeg_decoder* d)
 {
     const struct gj_geometry* g = &d->geo;
-    if ( d->out_mode != GJ_OUT_RGB || d->flipped || d->channel_remap ) return 0;
+    if ( d->out_mode != GJ_OUT_RGB || d->flipped || d->channel_remap || d->crop ) return 0;
     if ( d->stripes == 0 ) {
         const char* v = getenv("GPUJPEG_B200_STRIPES");
         const char* m = getenv("GPUJPEG_B200_STRIPE_MIN_BYTES");
@@ -597,7 +647,7 @@ static int split_by_segment_info(struct gpujpeg_decoder* d, const uint8_t* image
 {
     const struct gj_geometry* g = &d->geo;
     if ( !st->seginfo[0].pieces || g->seg_mcu <= 0 || st->restart_interval <= 0 || d->ignore_segment_info ) return 0;
-    for ( int k = 0; k < GJ_MAX_COMP; k++ )
+    for ( int k = 0; k < GJ_MAX_COMP && !d->crop; k++ )
         if ( d->force_lanes[k] ) return 0;   /* the self-synchronising kernel was asked for */
     if ( (size_t)g->seg_count * 4 > d->seg_off_size ) {
         gj_cuda_free(d->d_seg_off);
@@ -659,7 +709,7 @@ static int split_by_segment_info(struct gpujpeg_decoder* d, const uint8_t* image
             break;
         }
     }
-    if ( !wants_thread_per_segment(d, g, ecs_bytes) ) return 0;
+    if ( !d->crop && !wants_thread_per_segment(d, g, ecs_bytes) ) return 0;   /* (a cropped frame always takes that kernel) */
     *st = t;
     *pos = p;
     *adobe = ad;
@@ -875,7 +925,7 @@ static int size_output(struct gpujpeg_decoder* d, const struct gpujpeg_image_par
     const int n = 8 / d->scale;
     d->out_w = pi->width;
     d->out_h = pi->height;
-    d->out_size = d->scale == 1 ? g->raw_size : d->raw.size;
+    d->out_size = d->scale == 1 && !d->crop ? g->raw_size : d->raw.size;
     for ( int c = 0; c < g->comp_count; c++ ) {
         const int div_h = g->max_hs / g->comp[c].hs, div_v = g->max_vs / g->comp[c].vs;
         d->scomp[c] = g->comp[c];
@@ -888,6 +938,18 @@ static int size_output(struct gpujpeg_decoder* d, const struct gpujpeg_image_par
         return -1;
     }
     return 0;
+}
+
+/* dec_opt_crop: room for `pairs` {segment, blocks} pairs on the host and the device */
+static int grow_pick(struct gpujpeg_decoder* d, size_t pairs)
+{
+    if ( pairs * 8 > d->h_pick_size ) {
+        free(d->h_pick);
+        d->h_pick_size = 0;
+        if ( !(d->h_pick = (uint32_t*)malloc(pairs * 8)) ) return -1;
+        d->h_pick_size = pairs * 8;
+    }
+    return grow_dev((void**)&d->d_pick, &d->d_pick_size, pairs * 8);
 }
 
 /* Progressive (SOF2) frames, from the first SOS on: the same upload, K0 and host marker walk as a baseline frame, then per
@@ -985,6 +1047,24 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
 
     struct gj_prog_args* a = &d->last_prog;
     memset(a, 0, sizeof *a);
+    if ( d->crop ) {   /* every scan decodes the segments that hold the rectangle's blocks (gj_prog_crop_pick) */
+        size_t pairs = 0;
+        for ( int k = 0; k < st->scan_count; k++ )
+            pairs += (size_t)d->prog_scans[k].seg_count;
+        gj_crop_blocks(g, 8 / d->scale, d->crop_x, d->crop_y, d->crop_w, d->crop_h, d->crop_blk);
+        if ( grow_pick(d, pairs) ) {
+            GJ_ERR("Decoder allocation failed: %s\n", gj_cuda_last_error());
+            return GPUJPEG_ERROR;
+        }
+        int n = 0;
+        for ( int k = 0; k < st->scan_count; k++ ) {
+            a->pick_off[k] = n;
+            a->pick_n[k] = gj_prog_crop_pick(&d->prog_scans[k], st->scan[k].comp, d->crop_blk, d->h_pick + 2 * n);
+            n += a->pick_n[k];
+        }
+        if ( n && gj_cuda_memcpy_h2d_async(d->d_pick, d->h_pick, (size_t)n * 8, d->stream) ) return GPUJPEG_ERROR;
+        a->d_pick = d->d_pick;
+    }
     a->scans = d->prog_scans;
     a->scan_count = st->scan_count;
     a->d_luts = d->d_prog_luts;
@@ -1103,15 +1183,52 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         GJ_ERR("dec_opt_flipped is not supported together with dec_opt_scale.\n");
         return GPUJPEG_ERROR;
     }
-    if ( d->scale != d->scale_req ) d->last_valid = 0;   /* a resident re-run must not mix the buffers of two scales */
-    d->scale = d->scale_req;
+    if ( d->crop_req && d->flipped ) {
+        GJ_ERR("dec_opt_flipped is not supported together with dec_opt_crop.\n");
+        return GPUJPEG_ERROR;
+    }
+    /* the frame's scale and rectangle are committed to the decoder only once nothing below can refuse the frame: a refused
+     * frame leaves the last frame's state, which a resident re-run may still use, untouched */
+    const int scale = d->scale_req;
+    int crop = 0;
     struct gpujpeg_image_parameters pi;
     gpujpeg_image_set_default_parameters(&pi);
-    pi.width = (st.width + d->scale - 1) / d->scale;
-    pi.height = (st.height + d->scale - 1) / d->scale;
+    pi.width = (st.width + scale - 1) / scale;
+    pi.height = (st.height + scale - 1) / scale;
+    /* dec_opt_crop: the output is the rectangle, negotiated as an image of its size */
+    if ( d->crop_req ) {
+        if ( d->crop_rx >= pi.width || d->crop_ry >= pi.height || d->crop_rw > pi.width - d->crop_rx || d->crop_rh > pi.height - d->crop_ry ) {
+            GJ_ERR("Crop %dx%d+%d+%d does not lie inside the %dx%d output image.\n", d->crop_rw, d->crop_rh, d->crop_rx, d->crop_ry,
+                   pi.width, pi.height);
+            return GPUJPEG_ERROR;
+        }
+        /* a rectangle that is the whole image is the plain decode (the stripe pipeline included) */
+        if ( d->crop_rw < pi.width || d->crop_rh < pi.height ) crop = 1;
+        pi.width = d->crop_rw;
+        pi.height = d->crop_rh;
+    }
     int out_mode = choose_output(d, &st, &pi);
     if ( !out_mode ) return GPUJPEG_ERROR;
-    if ( d->scale > 1 && out_mode == GJ_OUT_RGB ) out_mode = GJ_OUT_GENERIC;   /* the fused kernels are full-size only */
+    if ( crop ) {
+        struct gj_raw_layout rl;
+        if ( gj_raw_layout_init(&rl, &pi) == 0 &&
+             ((rl.sampling[0].horizontal == 2 && (d->crop_rx & 1)) || (rl.sampling[0].vertical == 2 && (d->crop_ry & 1))) ) {
+            GJ_ERR("Crop %dx%d+%d+%d: pixel format %s needs an even %s.\n", d->crop_rw, d->crop_rh, d->crop_rx, d->crop_ry,
+                   gpujpeg_pixel_format_get_name(pi.pixel_format), (d->crop_rx & 1) ? "X" : "Y");
+            return GPUJPEG_ERROR;
+        }
+    }
+    /* from here on the decoder's buffers and output state change: the last frame can no longer be re-run (a frame that
+     * completes sets last_valid again) */
+    d->last_valid = 0;
+    d->scale = scale;
+    d->crop = crop;
+    d->crop_x = crop ? d->crop_rx : 0;
+    d->crop_y = crop ? d->crop_ry : 0;
+    d->crop_w = pi.width;
+    d->crop_h = pi.height;
+    /* the fused kernels are full-size only; a cropped RGB frame takes their window instances (launch_k4_crop) */
+    if ( d->scale > 1 && out_mode == GJ_OUT_RGB ) out_mode = GJ_OUT_GENERIC;
     struct gpujpeg_image_parameters pg = pi;   /* the coefficient planes: the stream's own size */
     pg.width = st.width;
     pg.height = st.height;
@@ -1132,7 +1249,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     }
     d->out_mode = out_mode;
     d->param_image.color_space = pi.color_space;
-    if ( (out_mode != GJ_OUT_RGB && gj_raw_layout_init(&d->raw, &pi)) || size_output(d, &pi) ) return GPUJPEG_ERROR;
+    if ( ((out_mode != GJ_OUT_RGB || d->crop) && gj_raw_layout_init(&d->raw, &pi)) || size_output(d, &pi) ) return GPUJPEG_ERROR;
     const struct gj_geometry* g = &d->geo;
 
     if ( st.progressive ) return decode_progressive(d, image, image_size, output, &st, &p, &pi, pos, adobe, early_cs, stats, t_begin);
@@ -1294,6 +1411,19 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     ha.d_coef = d->d_coef;
     ha.d_cext = d->d_cext;
     ha.d_tables = d->d_tab;
+    if ( d->crop ) {   /* K3 decodes the segments that hold the rectangle's blocks (gj_crop_pick), one thread per segment */
+        gj_crop_blocks(g, 8 / d->scale, d->crop_x, d->crop_y, d->crop_w, d->crop_h, d->crop_blk);
+        if ( grow_pick(d, (size_t)g->seg_count) ) {
+            GJ_ERR("Decoder allocation failed: %s\n", gj_cuda_last_error());
+            return GPUJPEG_ERROR;
+        }
+        int n = 0;
+        for ( int k = 0; k < g->scan_count; k++ )
+            n += gj_crop_pick(g, k, d->crop_blk, d->h_pick + 2 * n);
+        if ( n && gj_cuda_memcpy_h2d_async(d->d_pick, d->h_pick, (size_t)n * 8, d->stream) ) return GPUJPEG_ERROR;
+        ha.d_pick = d->d_pick;
+        ha.pick_count = n;
+    }
     d->last_args = ha;
     d->last_ecs_begin = ecs_begin;
     d->last_list_cap = list_cap;
@@ -1314,6 +1444,11 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         d->k3_parts = !(v && v[0] == '0');
     }
     const int k3_striped = striped && d->k3_parts && !resync && gj_huffman_decode_parts_eligible(&ha);
+    /* a cropped frame leaves blocks undecoded: their extent 0 makes them read as zero (the rule of gj_internal.h) */
+    if ( d->crop && gj_cuda_memset_async(d->d_cext, 0, g->coef_count / 64, d->stream) ) {
+        GJ_ERR("Decoder extent clear failed: %s\n", gj_cuda_last_error());
+        return GPUJPEG_ERROR;
+    }
     if ( !k3_striped && gj_launch_huffman_decode(&ha, d->stream) ) {
         GJ_ERR("Huffman decoder launch failed: %s\n", gj_cuda_last_error());
         return GPUJPEG_ERROR;
@@ -1418,6 +1553,22 @@ int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size, struct gpu
     return 0;
 }
 
+/* djpeg's -crop syntax "WxH+X+Y", decimal: v = {W, H, X, Y}; 0 on success */
+static int parse_crop(const char* p, int v[4])
+{
+    static const char seps[4] = {'x', '+', '+', 0};
+    for ( int i = 0; i < 4; i++ ) {
+        long n = 0;
+        const char* q = p;
+        while ( *q >= '0' && *q <= '9' && n < (1L << 30) )
+            n = n * 10 + (*q++ - '0');
+        if ( q == p || n >= (1L << 30) || *q != seps[i] ) return -1;
+        v[i] = (int)n;
+        p = q + 1;
+    }
+    return v[0] >= 1 && v[1] >= 1 ? 0 : -1;
+}
+
 /* [ref: src/gpujpeg_decoder.c:485-531] */
 int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt, const char* val)
 {
@@ -1480,6 +1631,23 @@ int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt,
         GJ_ERR("Unknown decoding scale: %s (1, 1/2, 1/4 or 1/8)\n", val);
         return GPUJPEG_ERROR;
     }
+    if ( strcmp(opt, GPUJPEG_DEC_OPT_CROP) == 0 ) {
+        if ( strcmp(val, "none") == 0 ) {
+            decoder->crop_req = 0;
+            return GPUJPEG_NOERR;
+        }
+        int v[4];
+        if ( parse_crop(val, v) ) {
+            GJ_ERR("Invalid crop: %s (WxH+X+Y with W, H >= 1, or none)\n", val);
+            return GPUJPEG_ERROR;
+        }
+        decoder->crop_rw = v[0];
+        decoder->crop_rh = v[1];
+        decoder->crop_rx = v[2];
+        decoder->crop_ry = v[3];
+        decoder->crop_req = 1;
+        return GPUJPEG_NOERR;
+    }
     if ( strcmp(opt, GPUJPEG_DEC_OPT_TGA_RLE_BOOL) == 0 || strcmp(opt, GPUJPEG_DEC_OPT_ALIGNMENT_BYTES_INT) == 0 ) {
         GJ_ERR("Decoder option %s is not implemented in this build.\n", opt);
         return GPUJPEG_ERROR;
@@ -1496,6 +1664,8 @@ void gpujpeg_decoder_print_options(void)
     printf("\t" GPUJPEG_DEC_OPT_CHANNEL_REMAP "=XYZ[W] - output channel mapping (as the encoder option)\n");
     printf("\t" GPUJPEG_DEC_OPT_SCALE "=[1|1/2|1/4|1/8] - decode to ceil(W*scale) x ceil(H*scale) pixels with libjpeg's reduced inverse "
            "DCTs (default: 1)\n");
+    printf("\t" GPUJPEG_DEC_OPT_CROP "=[WxH+X+Y|none] - decode only this rectangle of the (scaled) output image, Huffman-decoding only "
+           "the restart segments it covers (default: none)\n");
 }
 
 GPUJPEG_API int gpujpegx_decoder_used_segment_info(const struct gpujpeg_decoder* d)
@@ -1525,6 +1695,7 @@ GPUJPEG_API int gpujpegx_decoder_run_resident(struct gpujpeg_decoder* d, uint8_t
          gj_launch_marker_scan(d->d_file, d->last_ecs_begin, d->last_args.file_size, d->d_cta, d->d_list_pos, d->d_list_code,
                                d->d_list_cpos, d->last_list_cap, d->d_clean, d->d_mk, d->d_mk + 8, GJ_MK_OTHER_CAP, d->stream) )
         return -1;
+    if ( (stage_mask & 1) && d->crop && gj_cuda_memset_async(d->d_cext, 0, d->geo.coef_count / 64, d->stream) ) return -1;
     if ( (stage_mask & 1) && gj_launch_huffman_decode(&d->last_args, d->stream) ) return -1;
     if ( (stage_mask & 2) && launch_k4(d, d->last_tq, d_out ? d_out : d->d_raw, d->last_args.dequantize) ) return -1;
     return 0;

@@ -696,13 +696,14 @@ GJ_HD long gj_prog_block(const gj_prog_scan& S, int u, int i, int& ci)
     return S.blk_off[ci] + b;
 }
 
-/* Restart segment `seg` of a scan, clean bytes [cs, ce): every block of its units in coding order.  KIND is the scan's
+/* Restart segment `seg` of a scan, clean bytes [cs, ce): every block of its units in coding order (dec_opt_crop: of its
+ * first max_units units).  KIND is the scan's
  * GJ_PROG_* kind; `tab` the scan's tables by scan component (unused by DC refinements).  Predictors and the end-of-band
  * run start at zero, as after every restart marker.  Values go into the zig-zag coefficient buffer, raw (not dequantised),
  * and only inside the scan's band and the component's plane. */
 template <int KIND>
 GJ_HD void gj_prog_segment(const gj_prog_scan& S, const gj_dec_lut* tab, const uint32_t* clean, uint32_t cs, uint32_t ce, int seg,
-                           int16_t* coef)
+                           int16_t* coef, int max_units = 0x7FFFFFFF)
 {
     gj_prog_bits r;
     gj_prog_bits_init(r, clean, cs, ce);
@@ -711,7 +712,8 @@ GJ_HD void gj_prog_segment(const gj_prog_scan& S, const gj_dec_lut* tab, const u
         st.pred[c] = 0;
     st.eobrun = 0;
     const int u0 = seg * S.seg_units;
-    const int u1 = u0 + S.seg_units < S.units ? u0 + S.seg_units : S.units;
+    int u1 = u0 + S.seg_units < S.units ? u0 + S.seg_units : S.units;
+    if ( max_units < u1 - u0 ) u1 = u0 + max_units;
     const int ss = S.ss < 1 ? (KIND >= GJ_PROG_AC_FIRST ? 1 : 0) : S.ss > 63 ? 63 : S.ss;
     const int se = S.se > 63 ? 63 : S.se;
     for ( int u = u0; u < u1; u++ )

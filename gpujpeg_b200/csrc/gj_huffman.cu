@@ -1029,7 +1029,7 @@ struct SegOwners {
  * blocks out.  Fewer owners per warp make the warp's instruction stream shorter (the lock-step block loop runs as
  * long as its slowest lane, and every rarely-taken path is executed whenever ANY lane takes it), and that stream,
  * not the issue rate, is what bounds this kernel: 43 200 segments cannot fill the machine anyway. */
-template <bool DEQ, bool CLEAN>
+template <bool DEQ, bool CLEAN, bool PICK>
 __global__ void __launch_bounds__(HD_THREADS)
 k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file_end, const uint32_t* __restrict__ seg_off,
               int seg_count, int seg_mcu, const __grid_constant__ gj_huff_dec_args a, const __grid_constant__ SegOwners own,
@@ -1070,8 +1070,10 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
     if ( g0 >= g_end ) return;
     if ( !seg_off && !a.d_seg_tab && *a.d_error ) return;   // restart structure does not match the geometry: list ranks are meaningless
     constexpr bool clean = CLEAN;   // segment positions from K0's marker list, bits from its clean stream (own.cmp_words > 0)
-    const int g = g0 + lane;
-    const bool live = lane < SPW && g < g_end;
+    const int slot = g0 + lane;
+    const bool live = lane < SPW && slot < g_end;
+    /* PICK (dec_opt_crop): owner slots are entries {segment, blocks} of the pick list, seg_count is its length */
+    const int g = PICK ? (live ? (int)a.d_pick[2 * slot] : 0) : slot;
     const gj_scan_layout& L = a.lay;
     const int bpm = L.bpm;
     const bool general = !L.simple && L.interleaved;   // MCUs of several blocks per component
@@ -1083,6 +1085,7 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
         scan = scan_of_segment(L, g);
         const int s = g - L.scan_seg_begin[scan];
         nblocks = min(seg_mcu, L.scan_mcus[scan] - s * seg_mcu) * bpm;
+        if ( PICK ) nblocks = min(nblocks, (int)a.d_pick[2 * slot + 1]);
         // block index (in units of 64 coefficients) of the segment's first MCU; for single-component
         // scans the component plane is folded in here, for interleaved scans it is added per block
         mybase = s * seg_mcu + (L.interleaved ? 0 : L.blk_off[a.scan_comp[scan][0]]);
@@ -1117,7 +1120,9 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
             if ( ce < cs ) ce = cs;
         }
     }
-    const int max_blocks = seg_mcu * bpm;
+    /* PICK: a picked segment stops at its block count, so the warp stops after its longest one (without restart markers the
+     * segment is the whole scan) */
+    const int max_blocks = PICK ? __reduce_max_sync(FULL, live ? nblocks : 0) : seg_mcu * bpm;
     /* private block: 16-byte chunk c of lane L lives at chunk (c ^ (L & 7)) so that the warp-wide
      * 16-byte reads of the flush below are bank-conflict free */
     const int sw = lane & 7;
@@ -1232,6 +1237,19 @@ k_huff_decode(const uint8_t* __restrict__ file, const uint8_t* __restrict__ file
         if ( live ) src_init(r, file + start, file_end);
         decode_blocks(r);
     }
+}
+
+/* dec_opt_crop: a cropped frame decodes only some segments, but a restart marker with the wrong number anywhere in the frame
+ * must send it to resynchronisation as the full decode would (later segments are numbered differently there): the number
+ * of every marker in K0's list, one thread per segment */
+__global__ void __launch_bounds__(256) k_rst_check(const __grid_constant__ gj_huff_dec_args a)
+{
+    gj_pdl_wait();
+    const int g = blockIdx.x * 256 + threadIdx.x;
+    if ( g >= a.seg_count ) return;
+    const int scan = scan_of_segment(a.lay, g);
+    const int s = g - a.lay.scan_seg_begin[scan];
+    if ( s > 0 && a.d_list_code[a.first_rank[scan] + (uint32_t)s - 1u] != (uint8_t)(0xD0 + ((s - 1) & 7)) ) atomicExch(a.d_error, 1u);
 }
 
 /* zig-zag device coefficients -> natural order (debug / parity-test path only) */
@@ -1368,18 +1386,25 @@ extern "C" int gj_huffman_decode_parts_eligible(const struct gj_huff_dec_args* a
 
 extern "C" int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_stream_t stream)
 {
+    const bool pick = a->d_pick != nullptr;
     /* restart segments of at most 40 blocks (every RESTART_AUTO setting): several lanes per segment, self-synchronising
-     * (gj_huffdec.cu); longer segments: one thread per segment (below) */
-    if ( !a->force_thread_per_segment && gj_huffman_decode_sync_eligible(a) ) return gj_launch_huffman_decode_sync(a, stream);
+     * (gj_huffdec.cu); longer segments: one thread per segment (below).  A cropped frame always takes the latter. */
+    if ( !pick && !a->force_thread_per_segment && gj_huffman_decode_sync_eligible(a) ) return gj_launch_huffman_decode_sync(a, stream);
+    if ( pick && !a->d_seg_off && !a->d_seg_tab ) {
+        if ( gj_launch_pdl(k_rst_check, dim3((a->seg_count + 255) / 256), dim3(256), 0, stream, *a) != cudaSuccess ) return -1;
+        if ( a->pick_count == 0 ) return 0;
+    }
+    const int owners = pick ? a->pick_count : a->seg_count;
+    if ( pick && owners <= 0 ) return 0;
     /* segment owners per warp: few segments cannot fill the machine, so the shorter lock-step chains of fewer owners
      * win; many dense segments need the lanes (see the measurements at HD_SEGMENTS_PER_WARP).  With one scan per
      * component the luminance scan carries most of the bits and finishes last: it gets fewer owners per warp than
      * the chrominance scans. */
     SegOwners own;
-    const int spw_all = a->seg_count <= 8000 ? 4 : a->seg_count <= 24000 ? 8 : HD_SEGMENTS_PER_WARP;
-    own.segs0 = a->seg_count;
+    const int spw_all = owners <= 8000 ? 4 : owners <= 24000 ? 8 : HD_SEGMENTS_PER_WARP;
+    own.segs0 = owners;
     own.spw0 = own.spw1 = spw_all;
-    if ( a->lay.scan_count > 1 ) {
+    if ( a->lay.scan_count > 1 && !pick ) {
         /* measured, K3 in us for luminance/chrominance owners 16/16 | 8/32 | 4/32 (photo-like content; random content
          * prefers more owners at 8K: 519 | 564 | 910):  8K 189 | 175 | 225,  4K 113 | 99 | 89,  HD 111 | 95 | 83 */
         own.segs0 = a->lay.scan_seg_begin[1];
@@ -1387,18 +1412,19 @@ extern "C" int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_str
         own.spw1 = 32;
     }
     own.warps0 = (own.segs0 + own.spw0 - 1) / own.spw0;
-    const int warps = own.warps0 + (a->seg_count - own.segs0 + own.spw1 - 1) / own.spw1;
+    const int warps = own.warps0 + (owners - own.segs0 + own.spw1 - 1) / own.spw1;
     const dim3 grid((warps + HD_THREADS / 32 - 1) / (HD_THREADS / 32));
     /* bits from K0's clean stream wherever the segment positions come from its marker list and the frame is not dense: a
      * warp's segments staged in shared memory, the area 1.25 times the densest scan's average per warp (more would cost
      * CTAs per SM: 8K needs five per SM for one wave), a warp whose bytes do not fit reads the clean stream in global
-     * memory.  8K S-photo q75: K3 207 -> 174 us (H100 80GB HBM3, 400 W) */
+     * memory.  8K S-photo q75: K3 207 -> 174 us (H100 80GB HBM3, 400 W).  The picked segments of a warp of a cropped frame
+     * need not follow each other: the warp stages the clean bytes from its first to its last segment when they fit. */
     own.cmp_words = 0;
     if ( !a->d_seg_off && !a->d_seg_tab && a->d_clean && a->d_list_cpos ) {
         size_t cmp_bytes = 0;
         for ( int s = 0; s < a->lay.scan_count; s++ ) {
             const int segs = a->lay.scan_seg_begin[s + 1] - a->lay.scan_seg_begin[s];
-            const int spw = s < 1 || own.segs0 == a->seg_count ? own.spw0 : own.spw1;
+            const int spw = s < 1 || own.segs0 == owners ? own.spw0 : own.spw1;
             const size_t want = ((size_t)a->scan_bytes[s] / (size_t)(segs > 0 ? segs : 1) + 16) * (size_t)spw * 5 / 4 + 64;
             if ( want > cmp_bytes ) cmp_bytes = want;
         }
@@ -1412,22 +1438,35 @@ extern "C" int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_str
     int dev = 0;
     if ( cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 ) return -1;
     if ( !__atomic_load_n(&attr_done[dev], __ATOMIC_ACQUIRE) ) {
-        if ( cudaFuncSetAttribute(k_huff_decode<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(HD_THREADS / 32 * HD_CMP_MAX + 64)) != cudaSuccess ||
-             cudaFuncSetAttribute(k_huff_decode<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(HD_THREADS / 32 * HD_CMP_MAX + 64)) != cudaSuccess )
+        const int cmp_max = (int)(HD_THREADS / 32 * HD_CMP_MAX + 64);
+        if ( cudaFuncSetAttribute(k_huff_decode<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, cmp_max) != cudaSuccess ||
+             cudaFuncSetAttribute(k_huff_decode<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, cmp_max) != cudaSuccess ||
+             cudaFuncSetAttribute(k_huff_decode<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cmp_max) != cudaSuccess ||
+             cudaFuncSetAttribute(k_huff_decode<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cmp_max) != cudaSuccess )
             return -1;
         __atomic_store_n(&attr_done[dev], 1, __ATOMIC_RELEASE);
     }
     auto launch = [&](auto kernel) {
         gj_launch_pdl(kernel, dim3(grid), dim3(HD_THREADS), smem, stream, a->d_file, a->d_file + a->file_size, a->d_seg_off,
-                      a->seg_count, a->seg_mcu, *a, own, a->d_coef, a->d_cext, a->d_tables);
+                      owners, a->seg_mcu, *a, own, a->d_coef, a->d_cext, a->d_tables);
     };
-    if ( own.cmp_words ) {
-        if ( a->dequantize ) launch(k_huff_decode<true, true>);
-        else launch(k_huff_decode<false, true>);
+    if ( pick ) {
+        if ( own.cmp_words ) {
+            if ( a->dequantize ) launch(k_huff_decode<true, true, true>);
+            else launch(k_huff_decode<false, true, true>);
+        }
+        else {
+            if ( a->dequantize ) launch(k_huff_decode<true, false, true>);
+            else launch(k_huff_decode<false, false, true>);
+        }
+    }
+    else if ( own.cmp_words ) {
+        if ( a->dequantize ) launch(k_huff_decode<true, true, false>);
+        else launch(k_huff_decode<false, true, false>);
     }
     else {
-        if ( a->dequantize ) launch(k_huff_decode<true, false>);
-        else launch(k_huff_decode<false, false>);
+        if ( a->dequantize ) launch(k_huff_decode<true, false, false>);
+        else launch(k_huff_decode<false, false, false>);
     }
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

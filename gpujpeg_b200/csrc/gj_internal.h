@@ -176,6 +176,21 @@ int gj_raw_layout_init(struct gj_raw_layout* l, const struct gpujpeg_image_param
 int gj_geometry_init(struct gj_geometry* g, const struct gpujpeg_parameters* param,
                      const struct gpujpeg_image_parameters* param_image);
 
+/* dec_opt_crop: the blocks of every component plane that an output rectangle needs -- columns [bx0, bx1), rows [by0, by1).
+ * Output pixel (x, y) reads component c at sample (x / (max_hs / hs), y / (max_vs / vs)), n samples per block side (8, or
+ * 8 / scale for a scaled decode). */
+struct gj_blk_rect {
+    int bx0, by0, bx1, by1;
+};
+void gj_crop_blocks(const struct gj_geometry* g, int n, int x, int y, int w, int h, struct gj_blk_rect win[GJ_MAX_COMP]);
+/* The restart segments of a scan that hold a unit (MCU) of the rectangle [ux0, ux1) x [uy0, uy1) of its units_x-wide unit
+ * grid, seg_units units per segment, bpm blocks per unit: pairs {seg_base + segment, blocks to decode} in ascending order,
+ * the block count reaching up to and including the segment's last needed unit.  Returns the number of pairs. */
+int gj_crop_pick_units(int units_x, int units, int seg_units, int bpm, int ux0, int uy0, int ux1, int uy1, int seg_base,
+                       uint32_t* out);
+/* the pick list of baseline scan k (pairs as above, global segment numbers), from the blocks gj_crop_blocks gave */
+int gj_crop_pick(const struct gj_geometry* g, int k, const struct gj_blk_rect win[GJ_MAX_COMP], uint32_t* out);
+
 /* ---- codestream writer (gj_writer.c)  [ref: src/gpujpeg_writer.c] ---- */
 /* what a header may carry besides the coding parameters: orientation (SPIFF directory entry / Exif tag) and user Exif tags */
 struct gj_exif_tags;
@@ -409,6 +424,11 @@ struct gj_huff_dec_args {
     int16_t* d_coef;
     uint8_t* d_cext;            /* the extent of every block of d_coef (GJ_CEXT_FULL) */
     const struct gj_dev_dec_tables* d_tables;
+    /* dec_opt_crop: decode only the pick_count pairs {global segment, blocks} of d_pick (gj_crop_pick), one thread per
+     * segment; the caller clears d_cext first.  With positions from the marker list the launch also checks the number of
+     * every restart marker of the frame, as a full decode would.  NULL: every segment. */
+    const uint32_t* d_pick;
+    int pick_count;
 };
 int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_stream_t stream);
 int gj_huffman_decode_parts_eligible(const struct gj_huff_dec_args* a);   /* part_seg_lo / part_seg_hi may be used */
@@ -433,6 +453,10 @@ struct gj_prog_scan {
 /* scan k of a progressive stream on the frame geometry g (which must be the interleaved one if any scan interleaves);
  * 0 on success, -1 if the scan does not fit the geometry */
 int gj_prog_scan_init(const struct gj_geometry* g, const struct gj_stream* s, int k, int restart_interval, struct gj_prog_scan* out);
+/* dec_opt_crop: the pick list of progressive scan S (pairs as gj_crop_pick_units, segment numbers of the scan); comp[i] is the
+ * frame component of scan component i */
+int gj_prog_crop_pick(const struct gj_prog_scan* S, const int comp[GJ_MAX_COMP], const struct gj_blk_rect win[GJ_MAX_COMP],
+                      uint32_t* out);
 
 struct gj_prog_args {
     const struct gj_prog_scan* scans;   /* host array, scan_count entries */
@@ -449,6 +473,9 @@ struct gj_prog_args {
     int comp_count;
     int comp_blk_off[GJ_MAX_COMP];      /* first block of every component (dequantisation table qinv_zz[component]) */
     const struct gj_dev_dec_tables* d_tables;
+    /* dec_opt_crop: scan k decodes only the pairs {segment, blocks} d_pick[2 * pick_off[k] ..] (pick_n[k] of them); NULL: all */
+    const uint32_t* d_pick;
+    int pick_off[GJ_MAX_SCANS], pick_n[GJ_MAX_SCANS];
 };
 /* zero the coefficients, decode every scan in stream order, dequantise */
 int gj_launch_progressive_decode(const struct gj_prog_args* a, gj_stream_t stream);
@@ -474,6 +501,11 @@ int gj_launch_fdct_rgb_ss(const uint8_t* d_raw, int width, int height, int pitch
 int gj_launch_idct_rgb_ss(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], const int comp_tq[3],
                           uint8_t* d_raw, int width, int height, int pitch, int idct_flavour, int coef_dequantized,
                           const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
+/* dec_opt_crop: the fused kernels on the rectangle [x, x + w) x [y, y + h) of the width x height RGB image only, into d_out with
+ * pitch 3w (any sampling of comp; 4:4:4 takes the k_idct_rgb444 instance) */
+int gj_launch_idct_rgb_window(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], const int comp_tq[3],
+                              uint8_t* d_out, int width, int height, int x, int y, int w, int h, int idct_flavour, int coef_dequantized,
+                              const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
 
 /* K1 / K4 without colour transform, any pixel format gj_raw_layout_init describes, any sampling: one thread per 8x8
  * block reads / writes its samples straight from / to the raw image
@@ -482,14 +514,22 @@ int gj_launch_idct_rgb_ss(const int16_t* d_coef, const uint8_t* d_cext, const st
 int gj_launch_fdct_samples(const uint8_t* d_raw, const struct gj_raw_layout* raw, int16_t* d_coef, uint64_t* d_nzmask,
                            const struct gj_comp_geo* comp, int comp_count, const uint8_t* comp_tbl,
                            const struct gj_dev_enc_tables* h_tables, gj_stream_t stream);
+/* dec_opt_crop: K4 on a window -- only the blocks blk[c] of every component are transformed, and sample (sx, sy) of
+ * component c goes to (sx - ox[c], sy - oy[c]) of the raw image, kept where that lies inside comp[c].width x comp[c].height */
+struct gj_k4_window {
+    struct gj_blk_rect blk[GJ_MAX_COMP];
+    int ox[GJ_MAX_COMP], oy[GJ_MAX_COMP];
+};
 int gj_launch_idct_samples(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
                            const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int idct_flavour, int coef_dequantized,
-                           const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
+                           const struct gj_dev_dec_tables* h_tables, const struct gj_k4_window* win /* NULL: every block */,
+                           gj_stream_t stream);
 /* K4 of scaled decoding (dec_opt_scale): libjpeg's reduced inverse DCT, n = 4, 2 or 1 samples per block side (scale 1/2, 1/4,
  * 1/8), from RAW quantised coefficients; comp[c].width / height are the component's sample extents at that scale */
 int gj_launch_idct_scaled(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
                           const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int n,
-                          const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
+                          const struct gj_dev_dec_tables* h_tables, const struct gj_k4_window* win /* NULL: every block */,
+                          gj_stream_t stream);
 
 /* Generic pre-/post-processing pass (gj_convert.cu): raw image in any supported pixel format and colour space <-> the
  * component planes of the YCbCr JPEG (plane c at byte comp[c].blk_off * n * n, pitch comp[c].bcx * n, n samples per block
@@ -498,9 +538,10 @@ int gj_launch_idct_scaled(const int16_t* d_coef, const uint8_t* d_cext, const st
 int gj_launch_convert_in(const uint8_t* d_raw, const struct gj_raw_layout* raw, enum gpujpeg_pixel_format fmt, int color_space,
                          int color_space_internal, int width, int height, uint8_t* d_planes, size_t planes_size,
                          const struct gj_comp_geo* comp, int comp_count, int max_hs, int max_vs, gj_stream_t stream);
+/* (x0, y0): the image pixel that becomes the raw image's (0, 0) -- dec_opt_crop converts only its rectangle; (0, 0) otherwise */
 int gj_launch_convert_out(const uint8_t* d_planes, uint8_t* d_raw, const struct gj_raw_layout* raw, enum gpujpeg_pixel_format fmt,
                           int color_space, int color_space_internal, int width, int height, const struct gj_comp_geo* comp,
-                          int comp_count, int max_hs, int max_vs, int n, gj_stream_t stream);
+                          int comp_count, int max_hs, int max_vs, int n, int x0, int y0, gj_stream_t stream);
 /* enc/dec_opt_flipped: vertical flip of the (padded) component planes; enc/dec_opt_channel_remap: channel permutation of
  * the raw image in place.  gj_launch_channel_remap returns -2 when the channel count does not match the pixel format and
  * -3 for pixel formats with chroma subsampling [replaces ref: src/gpujpeg_preprocessor.cu:456-559] */

@@ -30,10 +30,14 @@ namespace {
 constexpr int PD_THREADS = 64;
 constexpr int DQ_THREADS = 256;
 
-template <int KIND>
+/* PICK (dec_opt_crop): thread i decodes entry i {segment, blocks} of the scan's pick list, and every thread below the scan's
+ * segment count checks the number of the restart marker in front of its segment, so that a wrong one anywhere in the scan
+ * is refused as in a full decode */
+template <int KIND, bool PICK>
 __global__ void __launch_bounds__(PD_THREADS)
 k_prog_decode(const __grid_constant__ gj_prog_scan S, const gj_dec_lut* __restrict__ luts, const uint32_t* __restrict__ clean,
-              const uint32_t* __restrict__ list_cpos, const uint8_t* __restrict__ list_code, uint32_t* error, int16_t* coef)
+              const uint32_t* __restrict__ list_cpos, const uint8_t* __restrict__ list_code, uint32_t* error, int16_t* coef,
+              const uint32_t* __restrict__ pick, int n_pick)
 {
     gj_pdl_wait();
     __shared__ gj_dec_lut s_tab[GJ_MAX_COMP];
@@ -45,7 +49,18 @@ k_prog_decode(const __grid_constant__ gj_prog_scan S, const gj_dec_lut* __restri
             dst[i] = __ldg(src + i);
         __syncthreads();
     }
-    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if constexpr ( PICK ) {
+        const int t = s;
+        if ( t > 0 && t < S.seg_count && list_code[S.first_rank + (uint32_t)t - 1u] != (uint8_t)(0xD0 + ((t - 1) & 7)) )
+            atomicExch(error, 1u);
+        if ( t >= n_pick ) return;
+        s = (int)pick[2 * t];
+        const uint32_t r = S.first_rank + (uint32_t)s;
+        const uint32_t ce = list_cpos[r], cs = s ? list_cpos[r - 1] : S.cbegin;
+        gj_prog_segment<KIND>(S, s_tab, clean, cs, ce > cs ? ce : cs, s, coef, (int)pick[2 * t + 1] / S.bpm);
+        return;
+    }
     if ( s >= S.seg_count ) return;
     const uint32_t r = S.first_rank + (uint32_t)s;   /* the marker that ends the segment */
     const uint32_t ce = list_cpos[r], cs = s ? list_cpos[r - 1] : S.cbegin;
@@ -93,26 +108,23 @@ extern "C" int gj_launch_progressive_decode(const struct gj_prog_args* a, gj_str
     }
     for ( int k = 0; k < a->scan_count; k++ ) {
         const gj_prog_scan& S = a->scans[k];
-        const dim3 grid((S.seg_count + PD_THREADS - 1) / PD_THREADS), block(PD_THREADS);
+        const uint32_t* pick = a->d_pick ? a->d_pick + 2 * (size_t)a->pick_off[k] : nullptr;
+        const int n_pick = a->d_pick ? a->pick_n[k] : 0;
+        const int threads = pick && n_pick > S.seg_count ? n_pick : S.seg_count;
+        const dim3 grid((threads + PD_THREADS - 1) / PD_THREADS), block(PD_THREADS);
         cudaError_t e;
+#define GJ_PD(KIND)                                                                                                                  \
+    (pick ? gj_launch_pdl(k_prog_decode<KIND, true>, grid, block, 0, stream, S, a->d_luts, a->d_clean, a->d_list_cpos, a->d_list_code, \
+                          a->d_error, a->d_coef, pick, n_pick)                                                                     \
+          : gj_launch_pdl(k_prog_decode<KIND, false>, grid, block, 0, stream, S, a->d_luts, a->d_clean, a->d_list_cpos,            \
+                          a->d_list_code, a->d_error, a->d_coef, pick, n_pick))
         switch ( S.kind ) {
-            case GJ_PROG_DC_FIRST:
-                e = gj_launch_pdl(k_prog_decode<GJ_PROG_DC_FIRST>, grid, block, 0, stream, S, a->d_luts, a->d_clean, a->d_list_cpos,
-                                  a->d_list_code, a->d_error, a->d_coef);
-                break;
-            case GJ_PROG_DC_REFINE:
-                e = gj_launch_pdl(k_prog_decode<GJ_PROG_DC_REFINE>, grid, block, 0, stream, S, a->d_luts, a->d_clean, a->d_list_cpos,
-                                  a->d_list_code, a->d_error, a->d_coef);
-                break;
-            case GJ_PROG_AC_FIRST:
-                e = gj_launch_pdl(k_prog_decode<GJ_PROG_AC_FIRST>, grid, block, 0, stream, S, a->d_luts, a->d_clean, a->d_list_cpos,
-                                  a->d_list_code, a->d_error, a->d_coef);
-                break;
-            default:
-                e = gj_launch_pdl(k_prog_decode<GJ_PROG_AC_REFINE>, grid, block, 0, stream, S, a->d_luts, a->d_clean, a->d_list_cpos,
-                                  a->d_list_code, a->d_error, a->d_coef);
-                break;
+            case GJ_PROG_DC_FIRST: e = GJ_PD(GJ_PROG_DC_FIRST); break;
+            case GJ_PROG_DC_REFINE: e = GJ_PD(GJ_PROG_DC_REFINE); break;
+            case GJ_PROG_AC_FIRST: e = GJ_PD(GJ_PROG_AC_FIRST); break;
+            default: e = GJ_PD(GJ_PROG_AC_REFINE); break;
         }
+#undef GJ_PD
         if ( e != cudaSuccess ) return -1;
     }
     if ( a->dequantize ) {

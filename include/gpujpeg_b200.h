@@ -493,6 +493,15 @@ GPUJPEG_API int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size
  * scaled frames (there is one arithmetic); dec_opt_flipped together with a scale is refused.  gpujpeg_decoder_get_image_info
  * still reports the stream's own size. */
 #define GPUJPEG_DEC_OPT_SCALE "dec_opt_scale"
+/* Extension of this build (not in the reference): region of interest.  "WxH+X+Y" (djpeg's -crop syntax, decimal, W, H >= 1)
+ * or "none" (default): the decoder returns rows Y..Y+H-1, pixels X..X+W-1 of the image it would return without the option
+ * (at dec_opt_scale, of the scaled image), byte for byte, in output->param_image and data_size, for every output type; a
+ * planar format's chroma plane is cut at its own sampling.  Only the restart segments that hold the rectangle's blocks are
+ * Huffman-decoded (a stream without restart markers up to the rectangle's last block), and only its blocks are transformed.
+ * Refused: a rectangle outside the image, an odd X for a pixel format with horizontally subsampled chroma (an odd Y for
+ * 420-u8-p0p1p2), dec_opt_flipped together with a crop.  dec_opt_huffman and dec_opt_huffman_lanes do not apply to
+ * cropped frames (one thread per restart segment).  gpujpeg_decoder_get_image_info still reports the stream's own size. */
+#define GPUJPEG_DEC_OPT_CROP "dec_opt_crop"
 GPUJPEG_API int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt, const char* val);
 GPUJPEG_API void gpujpeg_decoder_print_options(void);
 
