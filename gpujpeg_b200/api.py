@@ -101,6 +101,8 @@ def _load():
         "gpujpegx_decoder_run_resident": (ci, [vp, vp, ci]),
         "gpujpegx_decoder_get_coefficients": (ci, [vp, vp, cs]),
         "gpujpegx_decoder_used_segment_info": (ci, [vp]),
+        "gpujpegx_decoder_used_subsequences": (ci, [vp]),
+        "gpujpegx_decoder_subsequence_rounds": (ci, [vp]),
         "gpujpegx_batch_create": (vp, [C.POINTER(ci), ci]),
         "gpujpegx_batch_destroy": (None, [vp]),
         "gpujpegx_batch_device_count": (ci, [vp]),
@@ -294,9 +296,10 @@ class Encoder:
 class Decoder:
     """gpujpeg_decoder_create / gpujpeg_decoder_decode / gpujpeg_decoder_destroy"""
 
-    def __init__(self, stream=0, idct="int", scale="1", crop=None):
+    def __init__(self, stream=0, idct="int", scale="1", crop=None, huffman="auto"):
         """scale: "1", "1/2", "1/4" or "1/8" -- decode to ceil(W * scale) x ceil(H * scale) pixels (dec_opt_scale)
-        crop: (x, y, w, h) -- return only that rectangle of the (scaled) image (dec_opt_crop)"""
+        crop: (x, y, w, h) -- return only that rectangle of the (scaled) image (dec_opt_crop)
+        huffman: "auto", "thread_per_segment" or "subsequence" -- the Huffman decoder kernel (dec_opt_huffman)"""
         self._h = lib.gpujpeg_decoder_create(C.c_void_p(stream))
         if not self._h:
             raise GpuJpegError("gpujpeg_decoder_create failed (no CUDA device?)")
@@ -304,6 +307,8 @@ class Decoder:
             self.set_option("dec_opt_idct", idct)
         if scale != "1":
             self.set_option("dec_opt_scale", scale)
+        if huffman != "auto":
+            self.set_option("dec_opt_huffman", huffman)
         if crop is not None:
             x, y, w, h = (int(v) for v in crop)
             self.set_option("dec_opt_crop", "%dx%d+%d+%d" % (w, h, x, y))
@@ -352,6 +357,16 @@ class Decoder:
     def used_segment_info(self):
         """True if the last frame's scans were split by the stream's own segment-info tables (no marker scan on the device)"""
         return lib.gpujpegx_decoder_used_segment_info(self._h) == 1
+
+    def used_subsequences(self):
+        """True if the last frame's Huffman stage ran the sub-sequence kernel (restart segments of any length in parallel)"""
+        return lib.gpujpegx_decoder_used_subsequences(self._h) == 1
+
+    def subsequence_rounds(self):
+        """rounds the sub-sequence kernel needed to reach its fixed point on the last frame (129: a segment was finished by one
+        thread), None if the frame did not run it"""
+        r = lib.gpujpegx_decoder_subsequence_rounds(self._h)
+        return None if r < 0 else r
 
     def coefficients(self, width, height, sampling=(1, 1), interleaved=0):
         """coefficients of the last frame, natural order: (array, dequantized) -- with the integer IDCT flavour

@@ -54,6 +54,9 @@ struct gpujpeg_decoder {
     int flipped;                  /* dec_opt_flipped */
     unsigned channel_remap;       /* dec_opt_channel_remap: (count << 24) | selector nibbles, 0 = none */
     int thread_per_segment;       /* dec_opt_huffman=thread_per_segment */
+    int subsequence_req;          /* dec_opt_huffman=subsequence */
+    int used_subsequences;        /* the last frame's Huffman stage ran the sub-sequence kernel */
+    void* d_ss_scratch; size_t d_ss_scratch_size;   /* its per-segment and per-sub-sequence state */
     int force_lanes[GJ_MAX_COMP]; /* dec_opt_huffman_lanes: lanes per restart segment by scan, 0 = chosen from the frame's segment count */
     int sm_count;
     int ff_cs_itu601_is_709;      /* [ref: libgpujpeg/gpujpeg_decoder.h:95] */
@@ -213,6 +216,7 @@ int gpujpeg_decoder_destroy(struct gpujpeg_decoder* d)
     gj_cuda_free_host(d->h_raw);
     gj_cuda_free(d->d_prog_luts);
     gj_cuda_free(d->d_pick);
+    gj_cuda_free(d->d_ss_scratch);
     free(d->h_pick);
     free(d->prog_scans);
     free(d->h_prog_luts);
@@ -634,6 +638,20 @@ static int wants_thread_per_segment(const struct gpujpeg_decoder* d, const struc
            (many_segments && (bytes_per_block_x10 < 80 || bytes_per_block_x10 > 200));
 }
 
+/* The sub-sequence kernel (gj_huffscan.cu) for frames without restart markers -- what libjpeg, PIL and OpenCV write unless
+ * asked --: there every scan is one segment, and one thread per segment decodes it in seconds at 8K (DESIGN section 6).
+ * Streams with restart markers keep the choice above whatever their interval: whether the new kernel pays for few long
+ * segments has not been measured, and dec_opt_huffman=subsequence forces it.  Clean streams of 512 MB and more (bit positions
+ * past 32 bits) stay on the thread-per-segment kernel. */
+static int wants_subsequences(const struct gpujpeg_decoder* d, const struct gj_geometry* g, size_t ecs_bytes)
+{
+    if ( d->thread_per_segment || ecs_bytes >= ((size_t)1 << 29) ) return 0;
+    if ( d->subsequence_req ) return 1;
+    for ( int k = 0; k < GJ_MAX_COMP; k++ )
+        if ( d->force_lanes[k] ) return 0;
+    return g->restart_interval <= 0;
+}
+
 /* Segment info [ref: src/gpujpeg_reader.c:1168-1215]: a stream can carry, in front of every scan, the position of every
  * restart segment.  The reference's reader then splits the scan by that table instead of searching for markers; here the
  * search is K0's job on the device, and the table only pays when K3 runs one thread per segment on the file bytes (the
@@ -649,6 +667,7 @@ static int split_by_segment_info(struct gpujpeg_decoder* d, const uint8_t* image
     if ( !st->seginfo[0].pieces || g->seg_mcu <= 0 || st->restart_interval <= 0 || d->ignore_segment_info ) return 0;
     for ( int k = 0; k < GJ_MAX_COMP && !d->crop; k++ )
         if ( d->force_lanes[k] ) return 0;   /* the self-synchronising kernel was asked for */
+    if ( d->subsequence_req && !d->thread_per_segment ) return 0;   /* so was the sub-sequence kernel: it reads K0's clean stream */
     if ( (size_t)g->seg_count * 4 > d->seg_off_size ) {
         gj_cuda_free(d->d_seg_off);
         if ( d->h_seg_off ) gj_cuda_free_host(d->h_seg_off);
@@ -963,6 +982,7 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
     static const int comp_tq[GJ_MAX_COMP] = {0, 1, 2, 3};   /* qinv_zz[c]: the table component c latched at its first scan */
     d->last_valid = 0;
     d->used_segment_info = 0;
+    d->used_subsequences = 0;
     if ( (!d->prog_scans && !(d->prog_scans = (struct gj_prog_scan*)malloc(sizeof(struct gj_prog_scan) * GJ_MAX_SCANS))) ||
          (!d->h_prog_luts && !(d->h_prog_luts = (struct gj_dec_lut*)malloc(sizeof(struct gj_dec_lut) * GJ_MAX_SCANS * GJ_MAX_COMP))) ||
          (!d->d_prog_luts && gj_cuda_malloc((void**)&d->d_prog_luts, sizeof(struct gj_dec_lut) * GJ_MAX_SCANS * GJ_MAX_COMP)) ) {
@@ -1411,8 +1431,22 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     ha.d_coef = d->d_coef;
     ha.d_cext = d->d_cext;
     ha.d_tables = d->d_tab;
-    if ( d->crop ) {   /* K3 decodes the segments that hold the rectangle's blocks (gj_crop_pick), one thread per segment */
-        gj_crop_blocks(g, 8 / d->scale, d->crop_x, d->crop_y, d->crop_w, d->crop_h, d->crop_blk);
+    if ( !by_table && wants_subsequences(d, g, ecs_bytes) ) {
+        const int ctas = gj_subseq_grid();
+        const size_t need = ctas > 0 ? gj_subseq_scratch_bytes(g->seg_count, ecs_bytes, ctas) : 0;
+        if ( ctas <= 0 || grow_dev(&d->d_ss_scratch, &d->d_ss_scratch_size, need) ) {
+            GJ_ERR("Decoder allocation failed: %s\n", gj_cuda_last_error());
+            return GPUJPEG_ERROR;
+        }
+        ha.subsequence = 1;
+        ha.d_ss_scratch = d->d_ss_scratch;
+        ha.ss_scratch_bytes = d->d_ss_scratch_size;
+        ha.ecs_bytes = ecs_bytes;
+    }
+    /* a cropped frame: the blocks K4 transforms; K3 decodes the segments that hold them (gj_crop_pick), one thread per segment,
+     * unless the sub-sequence kernel decodes the whole frame */
+    if ( d->crop ) gj_crop_blocks(g, 8 / d->scale, d->crop_x, d->crop_y, d->crop_w, d->crop_h, d->crop_blk);
+    if ( d->crop && !ha.subsequence ) {
         if ( grow_pick(d, (size_t)g->seg_count) ) {
             GJ_ERR("Decoder allocation failed: %s\n", gj_cuda_last_error());
             return GPUJPEG_ERROR;
@@ -1478,6 +1512,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     }
     break;
   }
+    d->used_subsequences = ha.subsequence && !ha.d_seg_tab;
     output->metadata = &d->metadata;
 
     record_stats(d, output, &pi, stats, t_reader_ms, t_begin);
@@ -1583,8 +1618,15 @@ int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt,
         return GPUJPEG_NOERR;
     }
     if ( strcmp(opt, GPUJPEG_DEC_OPT_HUFFMAN) == 0 ) {
-        if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_AUTO) == 0 ) decoder->thread_per_segment = 0;
-        else if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_THREAD_PER_SEGMENT) == 0 ) decoder->thread_per_segment = 1;
+        if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_AUTO) == 0 ) decoder->thread_per_segment = decoder->subsequence_req = 0;
+        else if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_THREAD_PER_SEGMENT) == 0 ) {
+            decoder->thread_per_segment = 1;
+            decoder->subsequence_req = 0;
+        }
+        else if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_SUBSEQUENCE) == 0 ) {
+            decoder->thread_per_segment = 0;
+            decoder->subsequence_req = 1;
+        }
         else {
             GJ_ERR("Unknown Huffman decoder kernel: %s\n", val);
             return GPUJPEG_ERROR;
@@ -1671,6 +1713,17 @@ void gpujpeg_decoder_print_options(void)
 GPUJPEG_API int gpujpegx_decoder_used_segment_info(const struct gpujpeg_decoder* d)
 {
     return d && d->last_valid ? d->used_segment_info : -1;
+}
+
+GPUJPEG_API int gpujpegx_decoder_used_subsequences(const struct gpujpeg_decoder* d)
+{
+    return d && d->last_valid ? d->used_subsequences : -1;
+}
+
+GPUJPEG_API int gpujpegx_decoder_subsequence_rounds(struct gpujpeg_decoder* d)
+{
+    if ( !d || !d->last_valid || !d->used_subsequences ) return -1;
+    return gj_subseq_rounds(d->d_ss_scratch, d->stream);
 }
 
 /* ---- extension: re-run the GPU stages of the last decoded frame on the JPEG bytes already on the device ----

@@ -727,4 +727,211 @@ GJ_HD void gj_prog_segment(const gj_prog_scan& S, const gj_dec_lut* tab, const u
         }
 }
 
+/* ------------------------------------------------------------------------------------------- */
+/* baseline Huffman decoding by sub-sequences of a restart segment of any length: k_huff_decode_subseq (gj_huffscan.cu) */
+
+/* block number j (coding order) of the segment that starts at MCU first_mcu of scan `scan` -> block index in the
+ * coefficient buffer (the order segment_block() of gj_huffman.cu follows) */
+GJ_HD uint32_t gj_block_target(const gj_scan_layout& L, int scan, int first_mcu, int j)
+{
+    if ( !L.interleaved ) return (uint32_t)(L.blk_off[scan] + first_mcu + j);
+    if ( L.simple ) {
+        const int cps = L.comp_count;
+        const int mcu = j / cps;
+        return (uint32_t)(L.blk_off[j - mcu * cps] + first_mcu + mcu);
+    }
+    const int mcu = j / L.bpm, i = j - mcu * L.bpm;
+    const int m = first_mcu + mcu;
+    const int my = m / L.mcu_x, mx = m - my * L.mcu_x;
+    const int comp = L.idx_comp[i];
+    return (uint32_t)(L.blk_off[comp] + (my * L.comp_vs[comp] + L.idx_dy[i]) * L.bcx[comp] + mx * L.comp_hs[comp] + L.idx_dx[i]);
+}
+
+/* Where a walk stands: bit p relative to the segment's first clean bit (32 bits: a segment of up to 512 MB), zig-zag index k
+ * of the block being decoded (0: at the start of a block) and the block's index c inside the MCU.  Packed in 64 bits. */
+GJ_HD uint64_t gj_ss_pack(uint32_t p, uint32_t k, uint32_t c) { return (uint64_t)p | (uint64_t)k << 32 | (uint64_t)c << 40; }
+GJ_HD uint32_t gj_ss_p(uint64_t s) { return (uint32_t)s; }
+GJ_HD uint32_t gj_ss_k(uint64_t s) { return (uint32_t)(s >> 32) & 127u; }
+GJ_HD uint32_t gj_ss_c(uint64_t s) { return (uint32_t)(s >> 40) & 15u; }
+
+/* What a walk needs of a scan: the Huffman tables (DC, AC) and dequantisation table (zig-zag order) of every scan component,
+ * the scan component of every block of an MCU */
+struct gj_ss_scan {
+    const gj_dec_fast* fast[GJ_MAX_COMP][2];
+    const gj_dec_lut* lut[GJ_MAX_COMP][2];
+    const uint16_t* q[GJ_MAX_COMP];
+    uint8_t cimap[GJ_MAX_MCU_BLOCKS];
+    int bpm;
+};
+
+/* The bits of one segment, clean bytes [cs, ce) of K0's stream, through a two-word window; bits past ce read as zeros and
+ * no word behind the segment's last one is loaded. */
+struct gj_ss_bits {
+    const uint32_t* clean;
+    uint64_t bit0;   /* clean-stream bit of the segment's first bit */
+    uint32_t nbits;
+    uint64_t wi;     /* word of w0 */
+    uint32_t w0, w1;
+};
+GJ_HD void gj_ss_bits_init(gj_ss_bits& b, const uint32_t* clean, uint32_t cs, uint32_t ce)
+{
+    b.clean = clean;
+    b.bit0 = (uint64_t)cs * 8u;
+    b.nbits = ce > cs ? (ce - cs) * 8u : 0u;
+    b.wi = ~(uint64_t)0 >> 1;   /* no word yet (and wi + 1 of it is none either) */
+    b.w0 = b.w1 = 0;
+}
+/* the 32 bits from segment bit p on */
+GJ_HD uint32_t gj_ss_peek(gj_ss_bits& b, uint32_t p)
+{
+    if ( p >= b.nbits ) return 0u;
+    const uint64_t a = b.bit0 + p, wi = a >> 5;
+    if ( wi != b.wi ) {
+        b.w0 = wi == b.wi + 1 ? b.w1 : gj_prog_ld(b.clean + wi);
+        b.w1 = ((wi + 1) << 5) < b.bit0 + b.nbits ? gj_prog_ld(b.clean + wi + 1) : 0u;
+        b.wi = wi;
+    }
+    const uint32_t sh = (uint32_t)a & 31u, left = b.nbits - p;
+    uint32_t v = sh ? (b.w0 << sh) | (b.w1 >> (32u - sh)) : b.w0;
+    if ( left < 32u ) v &= ~(0xFFFFFFFFu >> left);
+    return v;
+}
+
+/* One symbol: the gj_dec_fast entry (zig-zag advance | bits to consume << 7 | value size << 16) for the 32 stream bits in
+ * `win`.  Codes no first- or second-level entry covers: canonical search in gj_dec_lut; a code no table holds consumes 16
+ * bits and reads as symbol 0 (end of block / DC size 0), as k_huff_decode reads it. */
+GJ_HD uint32_t gj_ss_entry(const gj_dec_fast& f, const gj_dec_lut& t, uint32_t win, bool ac)
+{
+    uint32_t e = gj_prog_ld(&f.e[win >> (32 - GJ_DEC_FAST_BITS)]);
+    if ( e & GJ_DEC_FAST_TOTAL_MASK ) return e;
+    if ( e ) {
+        e = gj_prog_ld(&f.sub[(e & 127u) - 1u][(win >> 16) & ((1u << (16 - GJ_DEC_FAST_BITS)) - 1u)]);
+        if ( e ) return e;
+    }
+    const uint32_t peek = win >> 16;
+    uint32_t l = GJ_DEC_FAST_BITS + 1;
+    for ( int q = GJ_DEC_FAST_BITS + 1; q < 16; q++ )
+        l += peek >= t.maxcode[q] ? 1u : 0u;
+    if ( peek >= t.maxcode[l] ) return (ac ? 64u : 1u) | 16u << GJ_DEC_FAST_TOTAL_SHIFT;
+    const uint32_t sym = t.vals[((int)(peek >> (16u - l)) + t.valoff[l]) & 255];
+    const uint32_t size = sym & 15u, run = sym >> 4;
+    const uint32_t kadv = !ac ? 1u : size ? run + 1u : run == 15u ? 16u : 64u;
+    return kadv | (l + size) << GJ_DEC_FAST_TOTAL_SHIFT | size << GJ_DEC_FAST_SIZE_SHIFT;
+}
+/* the value behind the code of entry e [ref: src/gpujpeg_huffman_cpu_decoder.c:169-204]; size 0 gives 0 */
+GJ_HD int gj_ss_value(uint32_t win, uint32_t e)
+{
+    const uint32_t total = (e >> GJ_DEC_FAST_TOTAL_SHIFT) & 31u, size = e >> GJ_DEC_FAST_SIZE_SHIFT;
+    const uint32_t mask = (1u << size) - 1u;
+    const uint32_t bits = (win >> (32u - total)) & mask;
+    return (int)bits - (int)(2u * bits <= mask ? mask : 0u);
+}
+
+/* The walk that tracks only the state, over the symbols that start in [p(st), p_end).  cross = the state at the first symbol
+ * boundary at or behind p_cross (what lies in front is warm-up, walked only to fall into step with the true symbol
+ * sequence); blocks = the blocks the symbols from there on finish, dc[] = the DC differences they decode, by scan component.
+ * Returns the state at the end. */
+GJ_HD uint64_t gj_ss_walk(const gj_ss_scan& S, gj_ss_bits& b, uint64_t st, uint32_t p_cross, uint32_t p_end, uint64_t& cross,
+                          int& blocks, int (&dc)[GJ_MAX_COMP])
+{
+    uint32_t p = gj_ss_p(st), k = gj_ss_k(st), c = gj_ss_c(st);
+    int nb = 0;
+    bool own = p >= p_cross;
+    cross = st;
+    for ( int i = 0; i < GJ_MAX_COMP; i++ )
+        dc[i] = 0;
+    while ( p < p_end ) {
+        if ( !own && p >= p_cross ) {
+            own = true;
+            cross = gj_ss_pack(p, k, c);
+        }
+        const uint32_t ci = S.cimap[c];
+        const uint32_t win = gj_ss_peek(b, p);
+        const uint32_t e = gj_ss_entry(*S.fast[ci][k != 0], *S.lut[ci][k != 0], win, k != 0);
+        if ( k == 0 && own ) dc[ci] += gj_ss_value(win, e);
+        p += (e >> GJ_DEC_FAST_TOTAL_SHIFT) & 31u;
+        k += e & 127u;
+        if ( k >= 64u ) {   /* end of block: EOB, or coefficient 63 reached */
+            k = 0;
+            nb += own ? 1 : 0;
+            c = c + 1u == (uint32_t)S.bpm ? 0u : c + 1u;
+        }
+    }
+    if ( !own ) cross = gj_ss_pack(p, k, c);   /* the warm-up's last symbol reached over the whole range */
+    blocks = nb;
+    return gj_ss_pack(p, k, c);
+}
+
+/* Coefficients [k_lo, k_hi) of a block, staged (zero between blocks), into the block in the coefficient buffer; the staging
+ * is left zero.  Whole 16-byte chunks where the range covers them. */
+GJ_HD void gj_ss_flush(int16_t* stage, int16_t* dst, uint32_t k_lo, uint32_t k_hi)
+{
+    for ( uint32_t i = k_lo >> 3; i < (k_hi + 7u) >> 3; i++ ) {
+        const uint32_t a = 8u * i, z = a + 8u;
+        if ( a >= k_lo && z <= k_hi ) {
+#if defined(__CUDA_ARCH__)
+            reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(stage)[i];
+            reinterpret_cast<uint4*>(stage)[i] = make_uint4(0u, 0u, 0u, 0u);
+#else
+            for ( uint32_t j = a; j < z; j++ ) {
+                dst[j] = stage[j];
+                stage[j] = 0;
+            }
+#endif
+        }
+        else {
+            for ( uint32_t j = a < k_lo ? k_lo : a; j < (z < k_hi ? z : k_hi); j++ ) {
+                dst[j] = stage[j];
+                stage[j] = 0;
+            }
+        }
+    }
+}
+
+/* The walk that writes, from the exact state st: block n of the segment (first_mcu = its first MCU, nblocks its blocks),
+ * pred[] the DC predictors there.  It takes the symbols that start before p_end and -- `last`: the segment's last
+ * sub-sequence -- goes on past the segment's end, where the bits are zeros, until the segment's blocks are done; it never
+ * writes a block behind them.  A block whose first symbols belong to the sub-sequence in front gets only the coefficients
+ * from the state's zig-zag index on, a block the next sub-sequence finishes only those in front of its index there: the two
+ * parts are disjoint and together the whole block.  The walk that decodes a block's DC writes its extent (GJ_CEXT_FULL).
+ * DEQ: coefficient * quantiser wrapped to int16, else the raw value. */
+template <bool DEQ>
+GJ_HD void gj_ss_write(const gj_ss_scan& S, gj_ss_bits& b, uint64_t st, uint32_t p_end, bool last, const gj_scan_layout& L, int scan,
+                       int first_mcu, int n, int nblocks, int (&pred)[GJ_MAX_COMP], int16_t* stage, int16_t* coef, uint8_t* cext)
+{
+    uint32_t p = gj_ss_p(st), k = gj_ss_k(st), c = gj_ss_c(st);
+    if ( n >= nblocks || (p >= p_end && !last) ) return;
+    uint32_t k_lo = k;
+    uint32_t ci = S.cimap[c];
+    while ( p < p_end || last ) {
+        const uint32_t win = gj_ss_peek(b, p);
+        const uint32_t e = gj_ss_entry(*S.fast[ci][k != 0], *S.lut[ci][k != 0], win, k != 0);
+        const int v = gj_ss_value(win, e);
+        const uint32_t kadv = e & 127u, idx = k + kadv - 1u;
+        if ( k == 0 ) {
+            pred[ci] += v;
+            stage[0] = (int16_t)(DEQ ? pred[ci] * (int)S.q[ci][0] : pred[ci]);
+        }
+        else if ( (e >> GJ_DEC_FAST_SIZE_SHIFT) && idx < 64u ) {
+            stage[idx] = (int16_t)(DEQ ? v * (int)S.q[ci][idx] : v);
+        }
+        p += (e >> GJ_DEC_FAST_TOTAL_SHIFT) & 31u;
+        k += kadv;
+        if ( k >= 64u ) {   /* end of block */
+            const uint32_t t = gj_block_target(L, scan, first_mcu, n);
+            gj_ss_flush(stage, coef + (size_t)t * 64, k_lo, 64u);
+            if ( k_lo == 0 ) cext[t] = GJ_CEXT_FULL;
+            k = k_lo = 0;
+            if ( ++n >= nblocks ) return;
+            c = c + 1u == (uint32_t)S.bpm ? 0u : c + 1u;
+            ci = S.cimap[c];
+        }
+    }
+    if ( k > k_lo ) {   /* the block the next sub-sequence finishes */
+        const uint32_t t = gj_block_target(L, scan, first_mcu, n);
+        gj_ss_flush(stage, coef + (size_t)t * 64, k_lo, k);
+        if ( k_lo == 0 ) cext[t] = GJ_CEXT_FULL;
+    }
+}
+
 #endif /* GJ_DEVICE_CUH */

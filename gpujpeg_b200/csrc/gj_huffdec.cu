@@ -91,23 +91,6 @@ struct SdParams {
     const gj_dev_dec_tables* tables;
 };
 
-/* block number j (coding order) of the segment that starts at MCU first_mcu of scan `scan` -> block index in the
- * coefficient buffer (the same mapping as segment_block() of gj_huffman.cu) */
-__device__ __forceinline__ uint32_t block_target(const gj_scan_layout& L, int scan, int first_mcu, int j)
-{
-    if ( !L.interleaved ) return (uint32_t)(L.blk_off[scan] + first_mcu + j);
-    if ( L.simple ) {
-        const int cps = L.comp_count;
-        const int mcu = j / cps;
-        return (uint32_t)(L.blk_off[j - mcu * cps] + first_mcu + mcu);
-    }
-    const int mcu = j / L.bpm, i = j - mcu * L.bpm;
-    const int m = first_mcu + mcu;
-    const int my = m / L.mcu_x, mx = m - my * L.mcu_x;
-    const int comp = L.idx_comp[i];
-    return (uint32_t)(L.blk_off[comp] + (my * L.comp_vs[comp] + L.idx_dy[i]) * L.bcx[comp] + mx * L.comp_hs[comp] + L.idx_dx[i]);
-}
-
 /* entry fields (gj_internal.h: struct gj_dec_fast) */
 constexpr uint32_t E_TOTAL = GJ_DEC_FAST_TOTAL_MASK;
 __device__ __forceinline__ uint32_t make_entry(uint32_t kadv, uint32_t total, uint32_t size)
@@ -610,7 +593,7 @@ __device__ __forceinline__ void run_units(const SdParams& P, const int scan, con
         uint8_t* const seg_ext = IL ? P.cext : P.cext + (size_t)L.blk_off[scan] + first_mcu;   // indexed as seg_glob, per block
         if ( IL ) {
             for ( int j = gl; j < nblocks; j += lanes )
-                tgt[j] = block_target(L, scan, first_mcu, j);
+                tgt[j] = gj_block_target(L, scan, first_mcu, j);
         }
         __syncwarp();   // staged bytes and tgt visible to the whole warp
         const uint32_t bits_all = len * 8u;

@@ -1381,11 +1381,20 @@ extern "C" int gj_launch_huffman_decode_sync(const struct gj_huff_dec_args* a, g
  * 4:4:4 frames with one scan per component, positions from the marker list */
 extern "C" int gj_huffman_decode_parts_eligible(const struct gj_huff_dec_args* a)
 {
-    return !a->force_thread_per_segment && gj_huffman_decode_sync_eligible(a) && !a->d_seg_tab && a->lay.simple && !a->lay.interleaved;
+    return !a->force_thread_per_segment && !a->subsequence && gj_huffman_decode_sync_eligible(a) && !a->d_seg_tab && a->lay.simple &&
+           !a->lay.interleaved;
 }
 
 extern "C" int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_stream_t stream)
 {
+    /* segments of any length, several threads per segment (gj_huffscan.cu): whole segments, a cropped frame included; the
+     * number of every restart marker is checked first, as a full decode by the kernels below would */
+    if ( a->subsequence && !a->d_seg_off && !a->d_seg_tab ) {
+        if ( a->seg_count > a->lay.scan_count &&
+             gj_launch_pdl(k_rst_check, dim3((a->seg_count + 255) / 256), dim3(256), 0, stream, *a) != cudaSuccess )
+            return -1;
+        return gj_launch_huffman_decode_subseq(a, a->d_ss_scratch, a->ss_scratch_bytes, a->ecs_bytes, stream);
+    }
     const bool pick = a->d_pick != nullptr;
     /* restart segments of at most 40 blocks (every RESTART_AUTO setting): several lanes per segment, self-synchronising
      * (gj_huffdec.cu); longer segments: one thread per segment (below).  A cropped frame always takes the latter. */

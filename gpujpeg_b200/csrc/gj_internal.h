@@ -429,8 +429,24 @@ struct gj_huff_dec_args {
      * every restart marker of the frame, as a full decode would.  NULL: every segment. */
     const uint32_t* d_pick;
     int pick_count;
+    /* the sub-sequence kernel (gj_huffscan.cu) for every scan: segments of any length, several threads per segment; positions
+     * from the marker list only.  d_ss_scratch holds gj_subseq_scratch_bytes(seg_count, ecs_bytes, gj_subseq_grid()) bytes.
+     * A cropped frame decodes whole segments then (d_pick is not used). */
+    int subsequence;
+    void* d_ss_scratch;
+    size_t ss_scratch_bytes, ecs_bytes;
 };
 int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_stream_t stream);
+/* sub-sequence kernel: bytes per sub-sequence (a tuning value; GPUJPEG_B200_SUBSEQ_BYTES overrides it for experiments), the
+ * smallest value the scratch is sized for, warm-up of a sub-sequence's first walk */
+#define GJ_SS_SUB_BYTES 32
+#define GJ_SS_MIN_BYTES 16
+#define GJ_SS_WARM_BITS 256
+size_t gj_subseq_scratch_bytes(int seg_count, size_t ecs_bytes, int grid_ctas);
+int gj_subseq_grid(void);   /* CTAs of its cooperative grid on the current device, -1 on error */
+int gj_subseq_rounds(const void* d_scratch, gj_stream_t stream);   /* rounds of the last launch on that scratch */
+int gj_launch_huffman_decode_subseq(const struct gj_huff_dec_args* a, void* d_scratch, size_t scratch_bytes, size_t ecs_bytes,
+                                    gj_stream_t stream);
 int gj_huffman_decode_parts_eligible(const struct gj_huff_dec_args* a);   /* part_seg_lo / part_seg_hi may be used */
 
 /* Progressive frames (gj_progressive.cu): one scan of a SOF2 frame as k_prog_decode sees it.  An interleaved scan (DC

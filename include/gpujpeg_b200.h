@@ -478,11 +478,18 @@ GPUJPEG_API int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size
 #define GPUJPEG_DEC_OPT_IDCT "dec_opt_idct"
 #define GPUJPEG_DEC_IDCT_VAL_INT "int"
 #define GPUJPEG_DEC_IDCT_VAL_FLOAT_GPUREF "float_gpuref"
-/* extension: which Huffman decoder kernel runs.  "auto" (default): several lanes per restart segment, self-synchronising,
- * for segments of at most 40 blocks, one thread per segment otherwise; "thread_per_segment": always the latter */
+/* extension: which Huffman decoder kernel runs on baseline scans.  "auto" (default): for frames without restart markers,
+ * sub-sequences of 32 bytes, one per thread, synchronised over the whole scan; otherwise several lanes per restart segment,
+ * self-synchronising, for segments of at most 40 blocks, one thread per segment for longer ones.  "thread_per_segment":
+ * always the latter two.  "subsequence": the sub-sequence kernel for every baseline scan.  Streams decoded from their
+ * segment-info tables and resynchronised streams take the thread-per-segment kernel; progressive scans their own.
+ * On damaged entropy-coded data the kernels can differ: the sub-sequence kernel reads the bits past a restart segment's end
+ * as zeros (as libjpeg does), the thread-per-segment kernel reads the bytes that follow the segment.  A code no Huffman table
+ * holds consumes 16 bits and reads as symbol 0 in every kernel. */
 #define GPUJPEG_DEC_OPT_HUFFMAN "dec_opt_huffman"
 #define GPUJPEG_DEC_HUFFMAN_VAL_AUTO "auto"
 #define GPUJPEG_DEC_HUFFMAN_VAL_THREAD_PER_SEGMENT "thread_per_segment"
+#define GPUJPEG_DEC_HUFFMAN_VAL_SUBSEQUENCE "subsequence"
 /* extension (tuning): lanes that share one restart segment in the self-synchronising decoder: 0 = chosen per scan from
  * the scan's bytes per segment (default), or 4, 8, 16, 32 for every scan */
 #define GPUJPEG_DEC_OPT_HUFFMAN_LANES "dec_opt_huffman_lanes"
@@ -497,10 +504,11 @@ GPUJPEG_API int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size
  * or "none" (default): the decoder returns rows Y..Y+H-1, pixels X..X+W-1 of the image it would return without the option
  * (at dec_opt_scale, of the scaled image), byte for byte, in output->param_image and data_size, for every output type; a
  * planar format's chroma plane is cut at its own sampling.  Only the restart segments that hold the rectangle's blocks are
- * Huffman-decoded (a stream without restart markers up to the rectangle's last block), and only its blocks are transformed.
+ * Huffman-decoded -- a frame the sub-sequence kernel decodes (dec_opt_huffman) is Huffman-decoded whole, in parallel --, and
+ * only its blocks are transformed.
  * Refused: a rectangle outside the image, an odd X for a pixel format with horizontally subsampled chroma (an odd Y for
- * 420-u8-p0p1p2), dec_opt_flipped together with a crop.  dec_opt_huffman and dec_opt_huffman_lanes do not apply to
- * cropped frames (one thread per restart segment).  gpujpeg_decoder_get_image_info still reports the stream's own size. */
+ * 420-u8-p0p1p2), dec_opt_flipped together with a crop.  dec_opt_huffman_lanes does not apply to cropped frames, and of
+ * dec_opt_huffman only the choice of the sub-sequence kernel (otherwise one thread per picked restart segment).  gpujpeg_decoder_get_image_info still reports the stream's own size. */
 #define GPUJPEG_DEC_OPT_CROP "dec_opt_crop"
 GPUJPEG_API int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt, const char* val);
 GPUJPEG_API void gpujpeg_decoder_print_options(void);

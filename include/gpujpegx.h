@@ -42,6 +42,12 @@ GPUJPEG_API int gpujpegx_decoder_get_coefficients(struct gpujpeg_decoder* decode
  * gpujpeg_parameters.segment_info of the encoder; reference: src/gpujpeg_reader.c:1168-1215) -- then no marker scan ran on
  * the device --, 0 if by the marker scan, -1 on error */
 GPUJPEG_API int gpujpegx_decoder_used_segment_info(const struct gpujpeg_decoder* decoder);
+/* 1 if the Huffman stage of the last decoded frame ran the sub-sequence kernel (dec_opt_huffman: restart segments of any
+ * length, several threads per segment), 0 if another kernel, -1 on error */
+GPUJPEG_API int gpujpegx_decoder_used_subsequences(const struct gpujpeg_decoder* decoder);
+/* measurement aid: rounds the sub-sequence kernel needed to reach its fixed point on the last frame (or on its last resident
+ * re-run); 129 when it finished a segment in one thread.  Waits for the decoder's stream.  -1 if the frame did not run it */
+GPUJPEG_API int gpujpegx_decoder_subsequence_rounds(struct gpujpeg_decoder* decoder);
 
 /* ---- batches of independent frames over several GPUs ---- */
 struct gpujpegx_batch;
