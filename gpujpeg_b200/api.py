@@ -296,10 +296,13 @@ class Encoder:
 class Decoder:
     """gpujpeg_decoder_create / gpujpeg_decoder_decode / gpujpeg_decoder_destroy"""
 
-    def __init__(self, stream=0, idct="int", scale="1", crop=None, huffman="auto"):
+    def __init__(self, stream=0, idct="int", scale="1", crop=None, huffman="auto", orientation="none"):
         """scale: "1", "1/2", "1/4" or "1/8" -- decode to ceil(W * scale) x ceil(H * scale) pixels (dec_opt_scale)
-        crop: (x, y, w, h) -- return only that rectangle of the (scaled) image (dec_opt_crop)
-        huffman: "auto", "thread_per_segment" or "subsequence" -- the Huffman decoder kernel (dec_opt_huffman)"""
+        crop: (x, y, w, h) -- return only that rectangle of the (scaled, oriented) image (dec_opt_crop)
+        huffman: "auto", "thread_per_segment" or "subsequence" -- the Huffman decoder kernel (dec_opt_huffman)
+        orientation: "none", "auto" (the stream's SPIFF / Exif orientation) or "0" / "90" / "180" / "270", optionally followed
+        by "-" -- turn the image clockwise, then mirror it horizontally (dec_opt_orientation); a quarter turn swaps the output's
+        width and height"""
         self._h = lib.gpujpeg_decoder_create(C.c_void_p(stream))
         if not self._h:
             raise GpuJpegError("gpujpeg_decoder_create failed (no CUDA device?)")
@@ -312,6 +315,8 @@ class Decoder:
         if crop is not None:
             x, y, w, h = (int(v) for v in crop)
             self.set_option("dec_opt_crop", "%dx%d+%d+%d" % (w, h, x, y))
+        if orientation != "none":
+            self.set_option("dec_opt_orientation", orientation)
 
     def set_option(self, key, val):
         if lib.gpujpeg_decoder_set_option(self._h, key.encode(), val.encode()) != 0:
@@ -328,7 +333,8 @@ class Decoder:
 
     def decode(self, jpeg, out=None):
         """jpeg: uint8 numpy array.  out: optional HxWx3 destination (numpy = custom host buffer, cuda tensor =
-        custom CUDA buffer).  Returns an HxWx3 uint8 numpy array (a copy) or `out`."""
+        custom CUDA buffer) of the output's shape (the oriented one under an orientation).  Returns an HxWx3 uint8 numpy
+        array (a copy) or `out`."""
         jpeg = np.ascontiguousarray(jpeg, np.uint8)
         if out is None:
             o = self.decode_raw(jpeg.ctypes.data, jpeg.size)

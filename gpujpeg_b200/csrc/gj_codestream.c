@@ -225,6 +225,60 @@ void gj_crop_blocks(const struct gj_geometry* g, int n, int x, int y, int w, int
     }
 }
 
+int gj_parse_orientation(const char* val, int* mode, int* rot, int* flip)
+{
+    static const char* const deg[4] = {"0", "90", "180", "270"};
+    if ( strcmp(val, "none") == 0 || strcmp(val, "auto") == 0 ) {
+        *mode = val[0] == 'a';
+        *rot = *flip = 0;
+        return 0;
+    }
+    for ( int r = 0; r < 4; r++ ) {
+        const size_t n = strlen(deg[r]);
+        if ( strncmp(val, deg[r], n) == 0 && (val[n] == '\0' || (val[n] == '-' && val[n + 1] == '\0')) ) {
+            *mode = 2;
+            *rot = r;
+            *flip = val[n] == '-';
+            return 0;
+        }
+    }
+    return -1;
+}
+
+int gj_orient_frame(int w, int h, int rot, int flip, const int* crop, int* ow, int* oh, struct gj_orient_map* m, int src[4])
+{
+    rot &= 3;
+    const int w2 = (rot & 1) ? h : w, h2 = (rot & 1) ? w : h;
+    const int cx = crop ? crop[0] : 0, cy = crop ? crop[1] : 0, cw = crop ? crop[2] : w2, ch = crop ? crop[3] : h2;
+    if ( cx < 0 || cy < 0 || cw < 1 || ch < 1 || cx >= w2 || cy >= h2 || cw > w2 - cx || ch > h2 - cy ) return -1;
+    /* oriented pixel (u, v): unmirror, u1 = f * u + u0, then undo the turn */
+    const int f = flip ? -1 : 1, u0 = flip ? w2 - 1 : 0;
+    struct gj_orient_map t;
+    memset(&t, 0, sizeof t);
+    switch ( rot ) {
+        case 0: t.sxx = f; t.sx0 = u0; t.syy = 1; break;                                 /* (u1, v) */
+        case 1: t.sxy = 1; t.syx = -f; t.sy0 = h - 1 - u0; break;                        /* (v, h - 1 - u1) */
+        case 2: t.sxx = -f; t.sx0 = w - 1 - u0; t.syy = -1; t.sy0 = h - 1; break;        /* (w - 1 - u1, h - 1 - v) */
+        default: t.sxy = -1; t.sx0 = w - 1; t.syx = f; t.sy0 = u0; break;                /* (w - 1 - v, u1) */
+    }
+    /* from the rectangle's origin */
+    t.sx0 += t.sxx * cx + t.sxy * cy;
+    t.sy0 += t.syx * cx + t.syy * cy;
+    /* the inverse of a signed permutation is its transpose */
+    t.oxx = t.sxx; t.oxy = t.syx; t.ox0 = -(t.sxx * t.sx0 + t.syx * t.sy0);
+    t.oyx = t.sxy; t.oyy = t.syy; t.oy0 = -(t.sxy * t.sx0 + t.syy * t.sy0);
+    const int ax = t.sx0, ay = t.sy0;   /* source of the rectangle's corners (0, 0) and (cw - 1, ch - 1) */
+    const int bx = t.sxx * (cw - 1) + t.sxy * (ch - 1) + t.sx0, by = t.syx * (cw - 1) + t.syy * (ch - 1) + t.sy0;
+    src[0] = ax < bx ? ax : bx;
+    src[1] = ay < by ? ay : by;
+    src[2] = (ax < bx ? bx - ax : ax - bx) + 1;
+    src[3] = (ay < by ? by - ay : ay - by) + 1;
+    *ow = w2;
+    *oh = h2;
+    *m = t;
+    return 0;
+}
+
 int gj_crop_pick_units(int units_x, int units, int seg_units, int bpm, int ux0, int uy0, int ux1, int uy1, int seg_base,
                        uint32_t* out)
 {

@@ -39,7 +39,7 @@ struct ConvertParams {
     int width, height;
     int cs;                 /* colour space of the raw image (enum gpujpeg_color_space) */
     int cs_internal;        /* colour space of the JPEG's components */
-    int x0, y0;             /* decode, dec_opt_crop: raw pixel (x, y) is image pixel (x0 + x, y0 + y) */
+    gj_orient_map map;      /* decode, dec_opt_crop / dec_opt_orientation: the image pixel of raw pixel (x, y) */
 };
 
 __constant__ int c_to_rgb[5][9] = {{0}, {0}, {298, 0, 409, 298, -100, -208, 298, 516, 0},
@@ -93,24 +93,18 @@ k_convert_in(const uint8_t* __restrict__ raw, uint8_t* __restrict__ planes, cons
             raw[p.off[0] + (size_t)y * p.pitch[0] + (size_t)x * p.xs[0] + p.alpha_off];
 }
 
-/* ORIGIN: a rectangle of the image from (p.x0, p.y0) on; the raw image's chroma grid keeps its phase, as x0 (y0) is even
- * wherever the pixel format subsamples horizontally (vertically) */
-template <bool ORIGIN>
-__global__ void __launch_bounds__(256)
-k_convert_out(const uint8_t* __restrict__ planes, uint8_t* __restrict__ raw, const __grid_constant__ ConvertParams p)
+/* raw pixel (x, y) from the samples c (plane sample k = get(k), k < jpeg_comps) of the image pixel it shows */
+template <class Get>
+__device__ __forceinline__ void put_pixel(const ConvertParams& p, uint8_t* __restrict__ raw, int x, int y, Get get)
 {
-    const int x = blockIdx.x * 256 + threadIdx.x, y = blockIdx.y;
-    if ( x >= p.width ) return;
-    const int ix = ORIGIN ? p.x0 + x : x, iy = ORIGIN ? p.y0 + y : y;   /* the image pixel */
     int c[3] = {0, 128, 128};
     const int colour_comps = p.jpeg_comps < 3 ? p.jpeg_comps : 3;
     for ( int k = 0; k < colour_comps; k++ )
-        c[k] = planes[p.poff[k] + (size_t)(iy / p.pdv[k]) * p.ppitch[k] + ix / p.pdh[k]];
+        c[k] = get(k);
     if ( p.jpeg_comps >= 3 ) cs_transform(p.cs_internal, p.cs, c);
     raw[p.off[0] + (size_t)y * p.pitch[0] + (size_t)x * p.xs[0]] = (uint8_t)c[0];
     if ( p.alpha_off )   /* the stream's fourth component, opaque without one */
-        raw[p.off[0] + (size_t)y * p.pitch[0] + (size_t)x * p.xs[0] + p.alpha_off] =
-            p.jpeg_comps == 4 ? planes[p.poff[3] + (size_t)(iy / p.pdv[3]) * p.ppitch[3] + ix / p.pdh[3]] : (uint8_t)0xFF;
+        raw[p.off[0] + (size_t)y * p.pitch[0] + (size_t)x * p.xs[0] + p.alpha_off] = p.jpeg_comps == 4 ? (uint8_t)get(3) : (uint8_t)0xFF;
     if ( p.raw_comps == 1 ) return;
     if ( p.uyvy ) {
         const int k = (x & 1) ? 2 : 1;
@@ -119,6 +113,52 @@ k_convert_out(const uint8_t* __restrict__ planes, uint8_t* __restrict__ raw, con
     else if ( x % p.rdh[1] == 0 && y % p.rdv[1] == 0 ) {
         raw[p.off[1] + (size_t)(y / p.rdv[1]) * p.pitch[1] + (size_t)(x / p.rdh[1]) * p.xs[1]] = (uint8_t)c[1];
         raw[p.off[2] + (size_t)(y / p.rdv[2]) * p.pitch[2] + (size_t)(x / p.rdh[2]) * p.xs[2]] = (uint8_t)c[2];
+    }
+}
+
+/* MAP: raw pixel (x, y) shows image pixel p.map(x, y) -- a rectangle of the image (dec_opt_crop; the raw image's chroma grid
+ * keeps its phase, as the origin is even wherever the pixel format subsamples horizontally (vertically)), a half turn or a mirror
+ * (dec_opt_orientation: never with a subsampled pixel format).  Quarter turns take k_convert_out_t. */
+template <bool MAP>
+__global__ void __launch_bounds__(256)
+k_convert_out(const uint8_t* __restrict__ planes, uint8_t* __restrict__ raw, const __grid_constant__ ConvertParams p)
+{
+    const int x = blockIdx.x * 256 + threadIdx.x, y = blockIdx.y;
+    if ( x >= p.width ) return;
+    const gj_orient_map& m = p.map;
+    const int ix = MAP ? m.sxx * x + m.sxy * y + m.sx0 : x, iy = MAP ? m.syx * x + m.syy * y + m.sy0 : y;   /* the image pixel */
+    put_pixel(p, raw, x, y, [&](int k) { return (int)planes[p.poff[k] + (size_t)(iy / p.pdv[k]) * p.ppitch[k] + ix / p.pdh[k]]; });
+}
+
+/* A quarter turn: consecutive raw pixels of a row show pixels of consecutive image rows.  A CTA converts a 32 x 32 tile of the
+ * raw image: it first loads the plane samples the tile shows, row by row of the planes, into shared memory, and reads them
+ * from there down the columns (33-byte rows spread a column over the banks). */
+constexpr int CT = 32;
+__global__ void __launch_bounds__(CT * 8)
+k_convert_out_t(const uint8_t* __restrict__ planes, uint8_t* __restrict__ raw, const __grid_constant__ ConvertParams p)
+{
+    __shared__ uint8_t s[GJ_MAX_COMP][CT][CT + 1];
+    const gj_orient_map& m = p.map;
+    const int x0 = blockIdx.x * CT, y0 = blockIdx.y * CT;
+    const int x1 = min(x0 + CT, p.width) - 1, y1 = min(y0 + CT, p.height) - 1;
+    /* the image pixels of the tile's corners bound the samples it shows */
+    const int ax = m.sxx * x0 + m.sxy * y0 + m.sx0, bx = m.sxx * x1 + m.sxy * y1 + m.sx0;
+    const int ay = m.syx * x0 + m.syy * y0 + m.sy0, by = m.syx * x1 + m.syy * y1 + m.sy0;
+    const int ix0 = min(ax, bx), iy0 = min(ay, by), ix1 = max(ax, bx), iy1 = max(ay, by);
+    const int t = threadIdx.y * CT + threadIdx.x;
+    for ( int k = 0; k < p.jpeg_comps; k++ ) {
+        const int px0 = ix0 / p.pdh[k], py0 = iy0 / p.pdv[k], nx = ix1 / p.pdh[k] - px0 + 1, ny = iy1 / p.pdv[k] - py0 + 1;
+        for ( int i = t; i < CT * CT; i += CT * 8 ) {
+            const int r = i / CT, q = i % CT;
+            if ( r < ny && q < nx ) s[k][r][q] = planes[p.poff[k] + (size_t)(py0 + r) * p.ppitch[k] + px0 + q];
+        }
+    }
+    __syncthreads();
+    const int x = x0 + threadIdx.x;
+    if ( x > x1 ) return;
+    for ( int y = y0 + threadIdx.y; y <= y1; y += 8 ) {
+        const int ix = m.sxx * x + m.sxy * y + m.sx0, iy = m.syx * x + m.syy * y + m.sy0;
+        put_pixel(p, raw, x, y, [&](int k) { return (int)s[k][iy / p.pdv[k] - iy0 / p.pdv[k]][ix / p.pdh[k] - ix0 / p.pdh[k]]; });
     }
 }
 
@@ -215,13 +255,13 @@ extern "C" int gj_launch_convert_in(const uint8_t* d_raw, const struct gj_raw_la
 extern "C" int gj_launch_convert_out(const uint8_t* d_planes, uint8_t* d_raw, const struct gj_raw_layout* raw,
                                      enum gpujpeg_pixel_format fmt, int color_space, int color_space_internal, int width,
                                      int height, const struct gj_comp_geo* comp, int comp_count, int max_hs, int max_vs, int n,
-                                     int x0, int y0, gj_stream_t stream)
+                                     const struct gj_orient_map* map, gj_stream_t stream)
 {
     ConvertParams p;
     if ( fill_params(&p, raw, fmt, color_space, color_space_internal, width, height, comp, comp_count, max_hs, max_vs, n) ) return -1;
-    p.x0 = x0;
-    p.y0 = y0;
-    if ( x0 || y0 ) k_convert_out<true><<<dim3((width + 255) / 256, height), 256, 0, stream>>>(d_planes, d_raw, p);
+    if ( map ) p.map = *map;
+    if ( map && map->sxx == 0 ) k_convert_out_t<<<dim3((width + CT - 1) / CT, (height + CT - 1) / CT), dim3(CT, 8), 0, stream>>>(d_planes, d_raw, p);
+    else if ( map ) k_convert_out<true><<<dim3((width + 255) / 256, height), 256, 0, stream>>>(d_planes, d_raw, p);
     else k_convert_out<false><<<dim3((width + 255) / 256, height), 256, 0, stream>>>(d_planes, d_raw, p);
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -488,7 +488,58 @@ struct FusedWin {
     int x, y, w, h;
     int strip0, row0;
     int bx0[3], bx1[3], by0[3], by1[3];
+    gj_orient_map m;   /* ORIENT instances: source pixel <-> output pixel */
 };
+
+/* dec_opt_orientation (ORIENT instances, always windowed).  ORIENT 1, a half turn or a mirror: the CTA keeps its strip, whose rows
+ * land on whole output rows.  ORIENT 2, a quarter turn: a strip would land on 8-pixel pieces of 512 output rows, so the CTA
+ * takes a tile 64 pixels wide and 64 * VS high (strip0 / row0 count tiles), whose columns land on output rows of 64 * VS
+ * pixels; its staging rows are QT_PAD bytes longer than the tile, so that reading a column of them spreads over the banks. */
+constexpr int QT_PX = 64;
+constexpr int QT_PAD = 4;
+
+/* Phase B of an ORIENT instance: the pixels of the CTA's part of the rectangle, source columns [xs, xe) and rows [ys, ye), land on
+ * the output rectangle that is their image under w.m; it is written output row by output row in groups of 4 pixels counted from
+ * the output's left edge, a group that lies inside and whose destination is 4-byte aligned as three words, the others byte by
+ * byte.  Every output pixel reads its source samples: fetch(row, lx, Y, Cb, Cr) as in win_phase_b. */
+template <class Fetch>
+__device__ __forceinline__ void orient_phase_b(const FusedWin& w, int x0, int y0, int vw, int vh, int nthreads, uint8_t* __restrict__ raw,
+                                               size_t pitch, Fetch fetch)
+{
+    const int xs = max(x0, w.x), xe = min(x0 + vw, w.x + w.w), ys = max(y0, w.y), ye = min(y0 + vh, w.y + w.h);
+    if ( xs >= xe || ys >= ye ) return;
+    const gj_orient_map& m = w.m;
+    const int ax = m.oxx * xs + m.oxy * ys + m.ox0, bx = m.oxx * (xe - 1) + m.oxy * (ye - 1) + m.ox0;
+    const int ay = m.oyx * xs + m.oyy * ys + m.oy0, by = m.oyx * (xe - 1) + m.oyy * (ye - 1) + m.oy0;
+    const int oxs = min(ax, bx), oxe = max(ax, bx) + 1, oys = min(ay, by), rows = max(ay, by) + 1 - oys;
+    const int ka = oxs >> 2, ng = ((oxe - 1) >> 2) - ka + 1;
+    for ( int g = threadIdx.x; g < rows * ng; g += nthreads ) {
+        const int row = g / ng, k = ka + g - row * ng;
+        const int oy = oys + row, first = 4 * k;
+        int r[4], gg[4], bb[4];
+#pragma unroll
+        for ( int j = 0; j < 4; j++ ) {
+            const int ox = min(max(first + j, oxs), oxe - 1);   // (pixels outside: any valid sample, not stored)
+            int cy, cb, cr;
+            fetch(m.syx * ox + m.syy * oy + m.sy0 - y0, m.sxx * ox + m.sxy * oy + m.sx0 - x0, cy, cb, cr);
+            gj_ycbcr_to_rgb_raw(cy, cb, cr, r[j], gg[j], bb[j]);
+        }
+        const uint32_t o[3] = {pack4_sat_u8(r[0], gg[0], bb[0], r[1]), pack4_sat_u8(gg[1], bb[1], r[2], gg[2]),
+                               pack4_sat_u8(bb[2], r[3], gg[3], bb[3])};
+        uint8_t* p = raw + (size_t)oy * pitch + (size_t)k * 12;
+        if ( first >= oxs && first + 4 <= oxe && (reinterpret_cast<uintptr_t>(p) & 3) == 0 ) {
+            uint32_t* q = reinterpret_cast<uint32_t*>(p);
+            q[0] = o[0];
+            q[1] = o[1];
+            q[2] = o[2];
+        }
+        else {
+#pragma unroll
+            for ( int i = 0; i < 12; i++ )
+                if ( first + i / 3 >= oxs && first + i / 3 < oxe ) p[i] = (uint8_t)(o[i >> 2] >> (8 * (i & 3)));
+        }
+    }
+}
 
 /* Phase B of a WIN instance.  Groups of 4 output pixels are counted from the rectangle's left edge, so that a group whose 4
  * pixels lie in this strip and whose destination is 4-byte aligned is stored as three words (every group of a row whose
@@ -554,26 +605,33 @@ __device__ __forceinline__ void idct_int_px(const uint32_t (&packed)[32], const 
 // FLAVOUR 0 = integer IDCT (gpujpeg_idct_cpu), 1 = float GPU-reference IDCT
 // DEQ     true  = coefficients are raw quantised values: multiply by the table here
 //         false = K3 already stored coefficient*quantiser wrapped to int16 (FLAVOUR 0 only)
-template <int VEC, int FLAVOUR, bool DEQ, bool WIN>
+// ORIENT 0 = as stored, 1 / 2 = dec_opt_orientation (see orient_phase_b; with WIN, VEC 4): a quarter turn (2) takes a tile of
+// 8 x 8 blocks, block b of a component at (b % 8, b / 8)
+template <int VEC, int FLAVOUR, bool DEQ, bool WIN, int ORIENT = 0>
 __global__ void __launch_bounds__(NT)
 k_idct_rgb444(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext, int bcx, int nblk, uint8_t* __restrict__ raw, int width, int height,
               size_t pitch, const __grid_constant__ IdctParams prm, const __grid_constant__ FusedWin w)
 {
     gj_pdl_wait();
-    __shared__ __align__(16) uint8_t s_pl[3 * K4_PLANE];
+    constexpr bool QT = ORIENT == 2;
+    constexpr int SP = QT ? QT_PX + QT_PAD : STRIP_PX;   // staging row pitch
+    constexpr int PLANE = QT ? QT_PX * SP : K4_PLANE;
+    __shared__ __align__(16) uint8_t s_pl[3 * PLANE];
 
-    const int bx0 = (WIN ? w.strip0 + (int)blockIdx.x : (int)blockIdx.x) * TB;
-    const int by = WIN ? w.row0 + (int)blockIdx.y : (int)blockIdx.y;
+    const int bx0 = (WIN ? w.strip0 + (int)blockIdx.x : (int)blockIdx.x) * (QT ? QT_PX / 8 : TB);
+    const int by = (WIN ? w.row0 + (int)blockIdx.y : (int)blockIdx.y) * (QT ? QT_PX / 8 : 1);   // (first) block row
     const int x0 = bx0 * 8;
-    const int vw = min(STRIP_PX, width - x0);
-    const int vh = min(8, height - by * 8);
+    const int vw = min(QT ? QT_PX : STRIP_PX, width - x0);
+    const int vh = min(QT ? QT_PX : 8, height - by * 8);
 
     /* phase A: one thread = one block of one component */
     {
         const int comp = threadIdx.x >> 6;
         const int b = threadIdx.x & 63;
-        const bool in = bx0 + b < bcx && (!WIN || (bx0 + b >= w.bx0[comp] && bx0 + b < w.bx1[comp]));
-        const size_t bi = (size_t)comp * nblk + (size_t)by * bcx + bx0 + b;
+        const int bx = bx0 + (QT ? (b & 7) : b), byb = by + (QT ? (b >> 3) : 0);
+        const bool in = bx < bcx && (!WIN || (bx >= w.bx0[comp] && bx < w.bx1[comp])) &&
+                        (!QT || (byb >= w.by0[comp] && byb < w.by1[comp] && byb * bcx < nblk));
+        const size_t bi = (size_t)comp * nblk + (size_t)byb * bcx + bx0 + (QT ? (b & 7) : b);
         const int ext = in ? __ldg(cext + bi) : 0;
         const bool head = __all_sync(0xFFFFFFFFu, ext <= 2);   // warp-uniform: a warp holds blocks of one component
         if ( in ) {
@@ -601,15 +659,33 @@ k_idct_rgb444(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
                     px[i] = pack4_sat_u8(GJ_RINT(GJ_FADD(f[4 * i], 128.0f)), GJ_RINT(GJ_FADD(f[4 * i + 1], 128.0f)),
                                          GJ_RINT(GJ_FADD(f[4 * i + 2], 128.0f)), GJ_RINT(GJ_FADD(f[4 * i + 3], 128.0f)));
             }
-            uint8_t* dst = s_pl + comp * K4_PLANE + b * 8;
+            if constexpr ( QT ) {   // (rows of SP bytes: 4-byte aligned)
+                uint32_t* dst = reinterpret_cast<uint32_t*>(s_pl + comp * PLANE + (b >> 3) * 8 * SP + (b & 7) * 8);
 #pragma unroll
-            for ( int r = 0; r < 8; r++ )
-                *reinterpret_cast<uint2*>(dst + r * STRIP_PX) = make_uint2(px[2 * r], px[2 * r + 1]);
+                for ( int r = 0; r < 8; r++ ) {
+                    dst[r * SP / 4] = px[2 * r];
+                    dst[r * SP / 4 + 1] = px[2 * r + 1];
+                }
+            }
+            else {
+                uint8_t* dst = s_pl + comp * K4_PLANE + b * 8;
+#pragma unroll
+                for ( int r = 0; r < 8; r++ )
+                    *reinterpret_cast<uint2*>(dst + r * STRIP_PX) = make_uint2(px[2 * r], px[2 * r + 1]);
+            }
         }
     }
     __syncthreads();
 
-    if constexpr ( WIN ) {
+    if constexpr ( ORIENT != 0 ) {
+        orient_phase_b(w, x0, by * 8, vw, vh, NT, raw, pitch, [&](int row, int lx, int& cy, int& cb, int& cr) {
+            cy = s_pl[row * SP + lx];
+            cb = s_pl[PLANE + row * SP + lx];
+            cr = s_pl[2 * PLANE + row * SP + lx];
+        });
+        return;
+    }
+    else if constexpr ( WIN ) {
         win_phase_b<8>(w, x0, by * 8, vw, vh, NT, raw, pitch, [&](int row, int lx, int& cy, int& cb, int& cr) {
             cy = s_pl[row * STRIP_PX + lx];
             cb = s_pl[K4_PLANE + row * STRIP_PX + lx];
@@ -652,7 +728,9 @@ k_idct_rgb444(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
 
 /* K4 with chroma subsampling: the mirror image of k_fdct_rgb_ss.  Every pixel takes the chrominance sample at
  * (x / HS, y / VS) -- sample replication, as the reference's postprocessor [ref: src/gpujpeg_postprocessor.cu:55-76]. */
-template <int HS, int VS, int VEC, int FLAVOUR, bool DEQ, bool WIN>
+/* ORIENT as k_idct_rgb444; a quarter turn (2) takes a tile of 8 / HS x 8 MCUs (64 x 64 * VS pixels): luminance block t at
+ * (t % 8, t / 8), chrominance block v of a component at (v % (8 / HS), v / (8 / HS)) */
+template <int HS, int VS, int VEC, int FLAVOUR, bool DEQ, bool WIN, int ORIENT = 0>
 __global__ void __launch_bounds__(TB * VS + 2 * TB / HS)
 k_idct_rgb_ss(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext, const __grid_constant__ SsGrid grid, uint8_t* __restrict__ raw, int width,
               int height, size_t pitch, const __grid_constant__ IdctParams prm, const __grid_constant__ FusedWin w)
@@ -660,22 +738,45 @@ k_idct_rgb_ss(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
     gj_pdl_wait();
     constexpr int NTS = TB * VS + 2 * TB / HS;
     constexpr int CB = TB / HS;
+    constexpr bool QT = ORIENT == 2;
     constexpr int CW = STRIP_PX / HS;                 // chrominance samples per strip row
-    __shared__ __align__(16) uint8_t s_y[8 * VS * STRIP_PX];
-    __shared__ __align__(16) uint8_t s_c[2][8 * CW];
+    constexpr int TW = QT ? QT_PX : STRIP_PX;         // pixels per row of the CTA's part
+    constexpr int SPY = QT ? QT_PX + QT_PAD : STRIP_PX, SPC = QT ? QT_PX / HS + QT_PAD : CW;   // staging row pitches
+    constexpr int CROWS = QT ? QT_PX : 8;             // chrominance rows of the CTA's part
+    __shared__ __align__(16) uint8_t s_y[CROWS * VS * SPY];
+    __shared__ __align__(16) uint8_t s_c[2][CROWS * SPC];
 
     const int sx = WIN ? w.strip0 + (int)blockIdx.x : (int)blockIdx.x, sy = WIN ? w.row0 + (int)blockIdx.y : (int)blockIdx.y;
-    const int bx0 = sx * TB;
+    const int bx0 = sx * (TW / 8);
     const int x0 = bx0 * 8;
-    const int y0 = sy * 8 * VS;
-    const int vw = min(STRIP_PX, width - x0);
-    const int vh = min(8 * VS, height - y0);
+    const int y0 = sy * CROWS * VS;
+    const int vw = min(TW, width - x0);
+    const int vh = min(CROWS * VS, height - y0);
 
     {
         int comp, bx, by;
         uint8_t* dst;
         int dpitch;
-        if ( threadIdx.x < TB * VS ) {
+        if constexpr ( QT ) {
+            constexpr int MX = QT_PX / 8 / HS;   // MCUs per tile row
+            const int t = threadIdx.x;
+            if ( t < TB * VS ) {
+                comp = 0;
+                bx = bx0 + (t & 7);
+                by = sy * 8 * VS + (t >> 3);
+                dst = s_y + (t >> 3) * 8 * SPY + (t & 7) * 8;
+                dpitch = SPY;
+            }
+            else {
+                const int u = t - TB * VS, v = u % CB;
+                comp = 1 + u / CB;
+                bx = sx * MX + v % MX;
+                by = sy * 8 + v / MX;
+                dst = s_c[comp - 1] + (v / MX) * 8 * SPC + (v % MX) * 8;
+                dpitch = SPC;
+            }
+        }
+        else if ( threadIdx.x < TB * VS ) {
             comp = 0;
             const int b = threadIdx.x & (TB - 1), byl = threadIdx.x / TB;
             bx = bx0 + b;
@@ -718,14 +819,31 @@ k_idct_rgb_ss(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
                     px[i] = pack4_sat_u8(GJ_RINT(GJ_FADD(f[4 * i], 128.0f)), GJ_RINT(GJ_FADD(f[4 * i + 1], 128.0f)),
                                          GJ_RINT(GJ_FADD(f[4 * i + 2], 128.0f)), GJ_RINT(GJ_FADD(f[4 * i + 3], 128.0f)));
             }
+            if constexpr ( QT ) {   // (rows of SPY / SPC bytes: 4-byte aligned)
 #pragma unroll
-            for ( int r = 0; r < 8; r++ )
-                *reinterpret_cast<uint2*>(dst + r * dpitch) = make_uint2(px[2 * r], px[2 * r + 1]);
+                for ( int r = 0; r < 8; r++ ) {
+                    reinterpret_cast<uint32_t*>(dst + r * dpitch)[0] = px[2 * r];
+                    reinterpret_cast<uint32_t*>(dst + r * dpitch)[1] = px[2 * r + 1];
+                }
+            }
+            else {
+#pragma unroll
+                for ( int r = 0; r < 8; r++ )
+                    *reinterpret_cast<uint2*>(dst + r * dpitch) = make_uint2(px[2 * r], px[2 * r + 1]);
+            }
         }
     }
     __syncthreads();
 
-    if constexpr ( WIN ) {
+    if constexpr ( ORIENT != 0 ) {
+        orient_phase_b(w, x0, y0, vw, vh, NTS, raw, pitch, [&](int row, int lx, int& cy, int& cb, int& cr) {
+            cy = s_y[row * SPY + lx];
+            cb = s_c[0][(row / VS) * SPC + lx / HS];
+            cr = s_c[1][(row / VS) * SPC + lx / HS];
+        });
+        return;
+    }
+    else if constexpr ( WIN ) {
         win_phase_b<8 * VS>(w, x0, y0, vw, vh, NTS, raw, pitch, [&](int row, int lx, int& cy, int& cb, int& cr) {
             cy = s_y[row * STRIP_PX + lx];
             cb = s_c[0][(row / VS) * CW + lx / HS];
@@ -1207,10 +1325,12 @@ extern "C" int gj_launch_idct_rgb_ss(const int16_t* d_coef, const uint8_t* d_cex
 }
 
 /* dec_opt_crop on the fused kernels: the rectangle [x, x + w) x [y, y + h) of the RGB image into d_out (pitch 3w); 4:4:4 when
- * every component is 1x1, else the chroma-subsampling instance */
+ * every component is 1x1, else the chroma-subsampling instance.  dec_opt_orientation: the ORIENT instances, `orient` mapping the
+ * rectangle to the output (h x w pixels, pitch 3h, for a quarter turn). */
 extern "C" int gj_launch_idct_rgb_window(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], const int comp_tq[3],
                                          uint8_t* d_out, int width, int height, int x, int y, int w, int h, int idct_flavour,
-                                         int coef_dequantized, const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
+                                         int coef_dequantized, const struct gj_orient_map* orient, const struct gj_dev_dec_tables* h_tables,
+                                         gj_stream_t stream)
 {
     IdctParams prm;
     for ( int c = 0; c < 3; c++ )
@@ -1219,14 +1339,18 @@ extern "C" int gj_launch_idct_rgb_window(const int16_t* d_coef, const uint8_t* d
     if ( w < 1 || h < 1 || x < 0 || y < 0 || x + w > width || y + h > height ) return -1;
     const int hs = comp[0].hs, vs = comp[0].vs;
     if ( comp[1].hs != 1 || comp[1].vs != 1 || comp[2].hs != 1 || comp[2].vs != 1 ) return -1;
+    const int quarter = orient && orient->sxx == 0;
+    /* the pixels a CTA covers: a 512-pixel strip of an MCU row, or a quarter turn's 64 x 64 * vs tile */
+    const int tw = quarter ? QT_PX : STRIP_PX, th = quarter ? QT_PX * vs : 8 * vs;
     FusedWin fw;
     memset(&fw, 0, sizeof fw);
     fw.x = x;
     fw.y = y;
     fw.w = w;
     fw.h = h;
-    fw.strip0 = x / STRIP_PX;
-    fw.row0 = y / (8 * vs);
+    fw.strip0 = x / tw;
+    fw.row0 = y / th;
+    if ( orient ) fw.m = *orient;
     for ( int c = 0; c < 3; c++ ) {
         const int dh = hs / comp[c].hs, dv = vs / comp[c].vs;
         fw.bx0[c] = x / dh / 8;
@@ -1234,20 +1358,35 @@ extern "C" int gj_launch_idct_rgb_window(const int16_t* d_coef, const uint8_t* d
         fw.by0[c] = y / dv / 8;
         fw.by1[c] = (y + h - 1) / dv / 8 + 1;
     }
-    const dim3 grid((x + w - 1) / STRIP_PX - fw.strip0 + 1, (y + h - 1) / (8 * vs) - fw.row0 + 1);
-    const size_t pitch = (size_t)w * 3;
+    const dim3 grid((x + w - 1) / tw - fw.strip0 + 1, (y + h - 1) / th - fw.row0 + 1);
+    const size_t pitch = (size_t)(quarter ? h : w) * 3;
+    /* O: 0 = as stored, 1 = a half turn or a mirror, 2 = a quarter turn */
+    const int o = !orient ? 0 : quarter ? 2 : 1;
     if ( hs == 1 && vs == 1 ) {
-#define GJ_K4W(F, D) gj_launch_pdl(k_idct_rgb444<4, F, D, true>, grid, dim3(NT), 0, stream, d_coef, d_cext, comp[0].bcx, comp[0].nblk, d_out, width, height, pitch, prm, fw)
+#define GJ_K4W2(F, D, O) gj_launch_pdl(k_idct_rgb444<4, F, D, true, O>, grid, dim3(NT), 0, stream, d_coef, d_cext, comp[0].bcx, comp[0].nblk, d_out, width, height, pitch, prm, fw)
+#define GJ_K4W(F, D)                  \
+    do {                              \
+        if ( o == 0 ) GJ_K4W2(F, D, 0);  \
+        else if ( o == 1 ) GJ_K4W2(F, D, 1); \
+        else GJ_K4W2(F, D, 2);        \
+    } while ( 0 )
         if ( idct_flavour == 0 && coef_dequantized ) GJ_K4W(0, false);
         else if ( idct_flavour == 0 ) GJ_K4W(0, true);
         else GJ_K4W(1, true);
 #undef GJ_K4W
+#undef GJ_K4W2
         return cudaGetLastError() == cudaSuccess ? 0 : -1;
     }
     SsGrid sg;
     ss_grid_rows(&sg, comp, 0, (comp[0].bcy + vs - 1) / vs, height);
-#define GJ_K4WS2(H, V, F, D) \
-    gj_launch_pdl(k_idct_rgb_ss<H, V, 4, F, D, true>, grid, dim3(TB * V + 2 * TB / H), 0, stream, d_coef, d_cext, sg, d_out, width, height, pitch, prm, fw)
+#define GJ_K4WS3(H, V, F, D, O) \
+    gj_launch_pdl(k_idct_rgb_ss<H, V, 4, F, D, true, O>, grid, dim3(TB * V + 2 * TB / H), 0, stream, d_coef, d_cext, sg, d_out, width, height, pitch, prm, fw)
+#define GJ_K4WS2(H, V, F, D)                   \
+    do {                                       \
+        if ( o == 0 ) GJ_K4WS3(H, V, F, D, 0);      \
+        else if ( o == 1 ) GJ_K4WS3(H, V, F, D, 1); \
+        else GJ_K4WS3(H, V, F, D, 2);               \
+    } while ( 0 )
 #define GJ_K4WS(H, V)                                                          \
     do {                                                                       \
         if ( idct_flavour == 0 && coef_dequantized ) GJ_K4WS2(H, V, 0, false); \
@@ -1260,6 +1399,7 @@ extern "C" int gj_launch_idct_rgb_window(const int16_t* d_coef, const uint8_t* d
     else return -1;
 #undef GJ_K4WS
 #undef GJ_K4WS2
+#undef GJ_K4WS3
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 

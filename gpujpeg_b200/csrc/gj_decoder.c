@@ -80,6 +80,11 @@ struct gpujpeg_decoder {
     struct gj_blk_rect crop_blk[GJ_MAX_COMP];
     uint32_t* d_pick; size_t d_pick_size;
     uint32_t* h_pick; size_t h_pick_size;
+    /* dec_opt_orientation: orient_mode 0 = none, 1 = auto (the stream's own), 2 = orient_rot / orient_flip; orient = the frame
+     * being / last decoded is turned or mirrored, by omap (which also maps a crop: d->crop_x.. are then the source rectangle) */
+    int orient_mode, orient_rot, orient_flip;
+    int orient;
+    struct gj_orient_map omap;
     struct gpujpeg_image_metadata metadata;
 
     struct gj_dev_dec_tables h_tab, h_tab_prev;
@@ -397,7 +402,7 @@ static int launch_k4_scaled(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_
         return -1;
     return gj_launch_convert_out(d->d_planes, d_out, &d->raw, d->param_image.pixel_format, d->param_image.color_space,
                                  d->param.color_space_internal, d->out_w, d->out_h, g->comp, g->comp_count, g->max_hs, g->max_vs, n,
-                                 0, 0, d->stream);
+                                 d->orient ? &d->omap : NULL, d->stream);
 }
 
 /* K4 of a cropped frame: the blocks of the rectangle only -- RGB through the window instances of the fused kernels, the stream's
@@ -414,7 +419,7 @@ static int launch_k4_crop(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_CO
     struct gj_comp_geo padded[GJ_MAX_COMP];
     if ( d->out_mode == GJ_OUT_RGB )   /* the fused kernels' window instances */
         return gj_launch_idct_rgb_window(d->d_coef, d->d_cext, g->comp, comp_tq, d_out, g->width, g->height, d->crop_x, d->crop_y, d->crop_w,
-                                         d->crop_h, d->idct_flavour, coef_dequantized, &d->h_tab, d->stream);
+                                         d->crop_h, d->idct_flavour, coef_dequantized, d->orient ? &d->omap : NULL, &d->h_tab, d->stream);
     const int direct = d->out_mode == GJ_OUT_SAMPLES;
     if ( direct ) {
         for ( int c = 0; c < g->comp_count; c++ ) {
@@ -434,7 +439,7 @@ static int launch_k4_crop(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_CO
     if ( rc || direct ) return rc;
     return gj_launch_convert_out(d->d_planes, d_out, &d->raw, d->param_image.pixel_format, d->param_image.color_space,
                                  d->param.color_space_internal, d->out_w, d->out_h, g->comp, g->comp_count, g->max_hs, g->max_vs, n,
-                                 d->crop_x, d->crop_y, d->stream);
+                                 &d->omap, d->stream);
 }
 
 /* K4 for the coder's geometry: the 4:4:4 kernel or the chroma-subsampling template instance */
@@ -455,9 +460,12 @@ static int launch_k4(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], 
             return -1;
         if ( d->flipped && gj_launch_flip_planes(d->d_planes, padded, g->comp_count, d->stream) ) return -1;
         return gj_launch_convert_out(d->d_planes, d_out, &d->raw, d->param_image.pixel_format, d->param_image.color_space,
-                                     d->param.color_space_internal,
-                                     g->width, g->height, g->comp, g->comp_count, g->max_hs, g->max_vs, 8, 0, 0, d->stream);
+                                     d->param.color_space_internal, d->out_w, d->out_h, g->comp, g->comp_count, g->max_hs, g->max_vs, 8,
+                                     d->orient ? &d->omap : NULL, d->stream);
     }
+    if ( d->orient )   /* the ORIENT instances of the fused kernels, on the whole image */
+        return gj_launch_idct_rgb_window(d->d_coef, d->d_cext, g->comp, comp_tq, d_out, g->width, g->height, 0, 0, g->width, g->height,
+                                         d->idct_flavour, coef_dequantized, &d->omap, &d->h_tab, d->stream);
     /* dec_opt_flipped on the fused path (see gpujpeg_decoder_decode): rows are written last to first */
     int pitch = g->pitch;
     if ( d->flipped ) {
@@ -471,12 +479,12 @@ static int launch_k4(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], 
                                  coef_dequantized, &d->h_tab, d->stream);
 }
 
-/* The stripe pipeline applies to what the fused RGB kernels write as they go: no flip, no channel remap (and no scaled
- * frame: those never take GJ_OUT_RGB). */
+/* The stripe pipeline applies to what the fused RGB kernels write as they go: no flip, no channel remap, no orientation (the rows of
+ * a turned image are not the stripes' rows) (and no scaled frame: those never take GJ_OUT_RGB). */
 static int stripes_usable(struct gpujpeg_decoder* d)
 {
     const struct gj_geometry* g = &d->geo;
-    if ( d->out_mode != GJ_OUT_RGB || d->flipped || d->channel_remap || d->crop ) return 0;
+    if ( d->out_mode != GJ_OUT_RGB || d->flipped || d->channel_remap || d->crop || d->orient ) return 0;
     if ( d->stripes == 0 ) {
         const char* v = getenv("GPUJPEG_B200_STRIPES");
         const char* m = getenv("GPUJPEG_B200_STRIPE_MIN_BYTES");
@@ -1001,6 +1009,7 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
          gj_reader_finish(st, adobe, d->verbose) )
         return GPUJPEG_ERROR;
     d->metadata = st->metadata;
+    if ( d->orient ) memset(&d->metadata.vals[GPUJPEG_METADATA_ORIENTATION], 0, sizeof d->metadata.vals[0]);   /* the pixels are upright */
     if ( st->color_space != early_cs ) {
         GJ_ERR("The stream's colour space (%s) is announced after its first scan header; not supported.\n",
                gpujpeg_color_space_get_name(st->color_space));
@@ -1207,15 +1216,29 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         GJ_ERR("dec_opt_flipped is not supported together with dec_opt_crop.\n");
         return GPUJPEG_ERROR;
     }
-    /* the frame's scale and rectangle are committed to the decoder only once nothing below can refuse the frame: a refused
-     * frame leaves the last frame's state, which a resident re-run may still use, untouched */
+    /* dec_opt_orientation: the stream's own orientation (SPIFF directory / Exif, read with the headers) or the option's */
+    int rot = d->orient_rot, oflip = d->orient_flip;
+    if ( d->orient_mode == 1 ) {
+        const int set = st.metadata.vals[GPUJPEG_METADATA_ORIENTATION].set;
+        rot = set ? (int)st.metadata.vals[GPUJPEG_METADATA_ORIENTATION].orient.rotation : 0;
+        oflip = set ? (int)st.metadata.vals[GPUJPEG_METADATA_ORIENTATION].orient.flip : 0;
+    }
+    const int orient = d->orient_mode != 0 && (rot != 0 || oflip != 0);
+    /* (the flip acts on the padded planes, which is no mirror of the image; see below) */
+    if ( orient && d->flipped ) {
+        GJ_ERR("dec_opt_flipped is not supported together with dec_opt_orientation.\n");
+        return GPUJPEG_ERROR;
+    }
+    /* the frame's scale, rectangle and orientation are committed to the decoder only once nothing below can refuse the frame: a
+     * refused frame leaves the last frame's state, which a resident re-run may still use, untouched */
     const int scale = d->scale_req;
     int crop = 0;
     struct gpujpeg_image_parameters pi;
     gpujpeg_image_set_default_parameters(&pi);
-    pi.width = (st.width + scale - 1) / scale;
-    pi.height = (st.height + scale - 1) / scale;
-    /* dec_opt_crop: the output is the rectangle, negotiated as an image of its size */
+    const int sw = (st.width + scale - 1) / scale, sh = (st.height + scale - 1) / scale;   /* the (scaled) image as stored */
+    pi.width = (rot & 1) ? sh : sw;   /* the output: a quarter turn swaps the sides */
+    pi.height = (rot & 1) ? sw : sh;
+    /* dec_opt_crop: the output is the rectangle (of the oriented image), negotiated as an image of its size */
     if ( d->crop_req ) {
         if ( d->crop_rx >= pi.width || d->crop_ry >= pi.height || d->crop_rw > pi.width - d->crop_rx || d->crop_rh > pi.height - d->crop_ry ) {
             GJ_ERR("Crop %dx%d+%d+%d does not lie inside the %dx%d output image.\n", d->crop_rw, d->crop_rh, d->crop_rx, d->crop_ry,
@@ -1229,6 +1252,18 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     }
     int out_mode = choose_output(d, &st, &pi);
     if ( !out_mode ) return GPUJPEG_ERROR;
+    /* the 2:1 chroma pairs of a turned or mirrored image of odd size are not the source's pairs turned */
+    if ( orient && (pi.pixel_format == GPUJPEG_422_U8_P1020 || pi.pixel_format == GPUJPEG_422_U8_P0P1P2 ||
+                    pi.pixel_format == GPUJPEG_420_U8_P0P1P2) ) {
+        GJ_ERR("dec_opt_orientation is not supported for pixel format %s (chroma subsampling).\n",
+               gpujpeg_pixel_format_get_name(pi.pixel_format));
+        return GPUJPEG_ERROR;
+    }
+    /* the output rectangle's map to the (scaled) image and the rectangle of the image it shows */
+    struct gj_orient_map omap;
+    int src[4], ow, oh;
+    const int rect[4] = {d->crop_rx, d->crop_ry, d->crop_rw, d->crop_rh};
+    if ( gj_orient_frame(sw, sh, orient ? rot : 0, orient ? oflip : 0, crop ? rect : NULL, &ow, &oh, &omap, src) ) return GPUJPEG_ERROR;
     if ( crop ) {
         struct gj_raw_layout rl;
         if ( gj_raw_layout_init(&rl, &pi) == 0 &&
@@ -1243,12 +1278,16 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     d->last_valid = 0;
     d->scale = scale;
     d->crop = crop;
-    d->crop_x = crop ? d->crop_rx : 0;
-    d->crop_y = crop ? d->crop_ry : 0;
-    d->crop_w = pi.width;
-    d->crop_h = pi.height;
+    d->crop_x = src[0];
+    d->crop_y = src[1];
+    d->crop_w = src[2];
+    d->crop_h = src[3];
+    d->orient = orient;
+    d->omap = omap;
     /* the fused kernels are full-size only; a cropped RGB frame takes their window instances (launch_k4_crop) */
     if ( d->scale > 1 && out_mode == GJ_OUT_RGB ) out_mode = GJ_OUT_GENERIC;
+    /* the sample kernels write blocks where they stand: a turned or mirrored frame takes the planes and the generic pass */
+    if ( orient && out_mode == GJ_OUT_SAMPLES ) out_mode = GJ_OUT_GENERIC;
     struct gpujpeg_image_parameters pg = pi;   /* the coefficient planes: the stream's own size */
     pg.width = st.width;
     pg.height = st.height;
@@ -1296,6 +1335,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     }   /* K0 path */
     if ( gj_reader_finish(&st, adobe, d->verbose) ) return GPUJPEG_ERROR;
     d->metadata = st.metadata;   /* handed out with the output [ref: src/gpujpeg_reader.c:1626-1636, src/gpujpeg_decoder.c:466] */
+    if ( d->orient ) memset(&d->metadata.vals[GPUJPEG_METADATA_ORIENTATION], 0, sizeof d->metadata.vals[0]);   /* the pixels are upright */
     if ( st.color_space != early_cs ) {
         GJ_ERR("The stream's colour space (%s) is announced after its first scan header; not supported.\n",
                gpujpeg_color_space_get_name(st.color_space));
@@ -1690,6 +1730,17 @@ int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt,
         decoder->crop_req = 1;
         return GPUJPEG_NOERR;
     }
+    if ( strcmp(opt, GPUJPEG_DEC_OPT_ORIENTATION) == 0 ) {
+        int mode, rot, flip;
+        if ( gj_parse_orientation(val, &mode, &rot, &flip) ) {
+            GJ_ERR("Invalid orientation: %s (none, auto, or 0, 90, 180 or 270 optionally followed by '-')\n", val);
+            return GPUJPEG_ERROR;
+        }
+        decoder->orient_mode = mode;
+        decoder->orient_rot = rot;
+        decoder->orient_flip = flip;
+        return GPUJPEG_NOERR;
+    }
     if ( strcmp(opt, GPUJPEG_DEC_OPT_TGA_RLE_BOOL) == 0 || strcmp(opt, GPUJPEG_DEC_OPT_ALIGNMENT_BYTES_INT) == 0 ) {
         GJ_ERR("Decoder option %s is not implemented in this build.\n", opt);
         return GPUJPEG_ERROR;
@@ -1708,6 +1759,8 @@ void gpujpeg_decoder_print_options(void)
            "DCTs (default: 1)\n");
     printf("\t" GPUJPEG_DEC_OPT_CROP "=[WxH+X+Y|none] - decode only this rectangle of the (scaled) output image, Huffman-decoding only "
            "the restart segments it covers (default: none)\n");
+    printf("\t" GPUJPEG_DEC_OPT_ORIENTATION "=[none|auto|<deg>[-]] - turn the output <deg> = 0, 90, 180 or 270 degrees clockwise, then "
+           "mirror it horizontally with '-'; auto: as the stream's SPIFF or Exif orientation says (default: none)\n");
 }
 
 GPUJPEG_API int gpujpegx_decoder_used_segment_info(const struct gpujpeg_decoder* d)

@@ -191,6 +191,21 @@ int gj_crop_pick_units(int units_x, int units, int seg_units, int bpm, int ux0, 
 /* the pick list of baseline scan k (pairs as above, global segment numbers), from the blocks gj_crop_blocks gave */
 int gj_crop_pick(const struct gj_geometry* g, int k, const struct gj_blk_rect win[GJ_MAX_COMP], uint32_t* out);
 
+/* dec_opt_orientation: the output pixel (ox, oy) -- counted from the output rectangle's origin -- shows the source pixel
+ * (sxx * ox + sxy * oy + sx0, syx * ox + syy * oy + sy0) of the unoriented (scaled) image; o.. is the inverse map, from a source
+ * pixel to its output pixel.  The matrices are signed permutations. */
+struct gj_orient_map {
+    int sxx, sxy, sx0, syx, syy, sy0;
+    int oxx, oxy, ox0, oyx, oyy, oy0;
+};
+/* value of dec_opt_orientation: "none" -> mode 0, "auto" -> mode 1, "<deg>[-]" (0, 90, 180, 270; '-' = mirrored) -> mode 2 with
+ * rot = deg / 90 and flip; 0 on success */
+int gj_parse_orientation(const char* val, int* mode, int* rot, int* flip);
+/* The w x h image turned rot quarter turns clockwise, then mirrored horizontally if flip: its size *ow x *oh; the map of the
+ * rectangle crop = {x, y, w, h} of it (NULL: all of it) and src = {x, y, w, h}, the rectangle of the w x h image it shows.
+ * Returns -1 (and leaves the outputs alone) if crop does not lie inside the oriented image. */
+int gj_orient_frame(int w, int h, int rot, int flip, const int* crop, int* ow, int* oh, struct gj_orient_map* m, int src[4]);
+
 /* ---- codestream writer (gj_writer.c)  [ref: src/gpujpeg_writer.c] ---- */
 /* what a header may carry besides the coding parameters: orientation (SPIFF directory entry / Exif tag) and user Exif tags */
 struct gj_exif_tags;
@@ -518,10 +533,11 @@ int gj_launch_idct_rgb_ss(const int16_t* d_coef, const uint8_t* d_cext, const st
                           uint8_t* d_raw, int width, int height, int pitch, int idct_flavour, int coef_dequantized,
                           const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
 /* dec_opt_crop: the fused kernels on the rectangle [x, x + w) x [y, y + h) of the width x height RGB image only, into d_out with
- * pitch 3w (any sampling of comp; 4:4:4 takes the k_idct_rgb444 instance) */
+ * pitch 3w (any sampling of comp; 4:4:4 takes the k_idct_rgb444 instance).  dec_opt_orientation: `orient` (NULL: none) maps the
+ * rectangle to the output, which is then h x w pixels (pitch 3h) for a quarter turn. */
 int gj_launch_idct_rgb_window(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], const int comp_tq[3],
                               uint8_t* d_out, int width, int height, int x, int y, int w, int h, int idct_flavour, int coef_dequantized,
-                              const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
+                              const struct gj_orient_map* orient, const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);
 
 /* K1 / K4 without colour transform, any pixel format gj_raw_layout_init describes, any sampling: one thread per 8x8
  * block reads / writes its samples straight from / to the raw image
@@ -554,10 +570,11 @@ int gj_launch_idct_scaled(const int16_t* d_coef, const uint8_t* d_cext, const st
 int gj_launch_convert_in(const uint8_t* d_raw, const struct gj_raw_layout* raw, enum gpujpeg_pixel_format fmt, int color_space,
                          int color_space_internal, int width, int height, uint8_t* d_planes, size_t planes_size,
                          const struct gj_comp_geo* comp, int comp_count, int max_hs, int max_vs, gj_stream_t stream);
-/* (x0, y0): the image pixel that becomes the raw image's (0, 0) -- dec_opt_crop converts only its rectangle; (0, 0) otherwise */
+/* map: the image pixel each raw pixel shows -- dec_opt_crop converts only its rectangle, dec_opt_orientation turns and mirrors
+ * (the raw image is then width x height of the oriented output); NULL: raw pixel (x, y) is image pixel (x, y) */
 int gj_launch_convert_out(const uint8_t* d_planes, uint8_t* d_raw, const struct gj_raw_layout* raw, enum gpujpeg_pixel_format fmt,
                           int color_space, int color_space_internal, int width, int height, const struct gj_comp_geo* comp,
-                          int comp_count, int max_hs, int max_vs, int n, int x0, int y0, gj_stream_t stream);
+                          int comp_count, int max_hs, int max_vs, int n, const struct gj_orient_map* map, gj_stream_t stream);
 /* enc/dec_opt_flipped: vertical flip of the (padded) component planes; enc/dec_opt_channel_remap: channel permutation of
  * the raw image in place.  gj_launch_channel_remap returns -2 when the channel count does not match the pixel format and
  * -3 for pixel formats with chroma subsampling [replaces ref: src/gpujpeg_preprocessor.cu:456-559] */

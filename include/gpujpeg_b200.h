@@ -510,6 +510,16 @@ GPUJPEG_API int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size
  * 420-u8-p0p1p2), dec_opt_flipped together with a crop.  dec_opt_huffman_lanes does not apply to cropped frames, and of
  * dec_opt_huffman only the choice of the sub-sequence kernel (otherwise one thread per picked restart segment).  gpujpeg_decoder_get_image_info still reports the stream's own size. */
 #define GPUJPEG_DEC_OPT_CROP "dec_opt_crop"
+/* Extension of this build (not in the reference): apply an orientation while decoding.  "none" (default): the image as stored.
+ * "<deg>[-]" (enc_metadata's grammar: 0, 90, 180 or 270, optionally followed by '-'): turn the image <deg> degrees clockwise,
+ * then mirror it horizontally if '-' -- the (rotation, flip) of struct gpujpeg_orientation; Exif orientation 6 is "90", 8
+ * "270", 5 "90-", 7 "270-".  "auto": the stream's own orientation (SPIFF directory entry or Exif tag); a stream without one
+ * decodes as "none".  A quarter turn swaps the output's width and height; the orientation applies after dec_opt_scale, and the
+ * dec_opt_crop rectangle is given in the oriented image.  output->param_image describes the oriented output, and when an
+ * orientation other than the identity was applied output->metadata reports no orientation (the pixels are upright);
+ * gpujpeg_decoder_get_image_info2 still reports the stream as stored.  Refused for a frame it turns or mirrors: together with
+ * dec_opt_flipped, and pixel formats with chroma subsampling (422-u8-p1020, 422-u8-p0p1p2, 420-u8-p0p1p2). */
+#define GPUJPEG_DEC_OPT_ORIENTATION "dec_opt_orientation"
 GPUJPEG_API int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt, const char* val);
 GPUJPEG_API void gpujpeg_decoder_print_options(void);
 
