@@ -11,6 +11,7 @@ from .api import (  # noqa: F401
     GpuJpegError,
     ImageParameters,
     Parameters,
+    Transcoder,
     lib,
     library_path,
     version,

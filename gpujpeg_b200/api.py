@@ -103,6 +103,10 @@ def _load():
         "gpujpegx_decoder_used_segment_info": (ci, [vp]),
         "gpujpegx_decoder_used_subsequences": (ci, [vp]),
         "gpujpegx_decoder_subsequence_rounds": (ci, [vp]),
+        "gpujpegx_transcoder_create": (vp, [vp]),
+        "gpujpegx_transcoder_destroy": (None, [vp]),
+        "gpujpegx_transcoder_set_option": (ci, [vp, C.c_char_p, C.c_char_p]),
+        "gpujpegx_transcode": (ci, [vp, vp, cs, C.POINTER(vp), C.POINTER(cs)]),
         "gpujpegx_batch_create": (vp, [C.POINTER(ci), ci]),
         "gpujpegx_batch_destroy": (None, [vp]),
         "gpujpegx_batch_device_count": (ci, [vp]),
@@ -394,6 +398,43 @@ class Decoder:
     def close(self):
         if self._h:
             lib.gpujpeg_decoder_destroy(self._h)
+            self._h = None
+
+    __del__ = close
+
+
+class Transcoder:
+    """gpujpegx_transcoder_*: lossless JPEG-to-JPEG rewrite on the GPU (include/gpujpegx.h) -- the same quantised coefficients as
+    one baseline frame with the restart interval and Huffman tables asked for, optionally turned and mirrored"""
+
+    def __init__(self, stream=0, transform="none", restart="auto", huffman="standard", perfect=False):
+        """transform: "none", "auto" (the stream's SPIFF / Exif orientation) or "0" / "90" / "180" / "270", optionally followed by
+        "-" -- turn clockwise, then mirror horizontally (tran_opt_transform).  restart: "auto" or the interval in MCUs (0: no
+        markers).  huffman: "standard" (Annex K) or "optimized" (fitted to the frame).  perfect: refuse frames whose partial edge
+        iMCUs would move instead of dropping them."""
+        self._h = lib.gpujpegx_transcoder_create(C.c_void_p(stream))
+        if not self._h:
+            raise GpuJpegError("gpujpegx_transcoder_create failed (no CUDA device?)")
+        self.set_option("tran_opt_transform", transform)
+        self.set_option("tran_opt_restart", str(restart))
+        self.set_option("tran_opt_huffman", huffman)
+        self.set_option("tran_opt_perfect", "1" if perfect else "0")
+
+    def set_option(self, key, val):
+        if lib.gpujpegx_transcoder_set_option(self._h, key.encode(), val.encode()) != 0:
+            raise GpuJpegError("gpujpegx_transcoder_set_option(%s, %s) failed" % (key, val))
+
+    def transcode(self, jpeg):
+        """jpeg: uint8 numpy array.  Returns the rewritten JPEG as numpy uint8 (a copy)."""
+        jpeg = np.ascontiguousarray(jpeg, np.uint8)
+        out, size = C.c_void_p(), C.c_size_t()
+        if lib.gpujpegx_transcode(self._h, jpeg.ctypes.data, jpeg.size, C.byref(out), C.byref(size)) != 0:
+            raise GpuJpegError("gpujpegx_transcode failed")
+        return np.ctypeslib.as_array((C.c_uint8 * size.value).from_address(out.value)).copy()
+
+    def close(self):
+        if self._h:
+            lib.gpujpegx_transcoder_destroy(self._h)
             self._h = None
 
     __del__ = close

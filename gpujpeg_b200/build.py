@@ -17,8 +17,10 @@ OBJDIR = os.path.join(HERE, "build")
 SONAME = "libgpujpeg.so.0"
 LIB = os.path.join(LIBDIR, SONAME)
 
-C_SOURCES = ["gj_tables.c", "gj_codestream.c", "gj_common.c", "gj_imageio.c", "gj_exif.c", "gj_encoder.c", "gj_decoder.c", "gj_batch.c"]
-CU_SOURCES = ["gj_cuda_util.cu", "gj_dct.cu", "gj_huffman.cu", "gj_huffdec.cu", "gj_huffscan.cu", "gj_markers.cu", "gj_convert.cu", "gj_progressive.cu"]
+C_SOURCES = ["gj_tables.c", "gj_codestream.c", "gj_common.c", "gj_imageio.c", "gj_exif.c", "gj_encoder.c", "gj_decoder.c", "gj_batch.c",
+             "gj_transcoder.c"]
+CU_SOURCES = ["gj_cuda_util.cu", "gj_dct.cu", "gj_huffman.cu", "gj_huffdec.cu", "gj_huffscan.cu", "gj_markers.cu", "gj_convert.cu", "gj_progressive.cu",
+              "gj_transcode.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 

@@ -279,6 +279,114 @@ int gj_orient_frame(int w, int h, int rot, int flip, const int* crop, int* ow, i
     return 0;
 }
 
+static void plan_geometry(struct gj_geometry* g, int w, int h, int comp_count, const int* hs, const int* vs, int il)
+{
+    struct gpujpeg_parameters p;
+    struct gpujpeg_image_parameters pi;
+    memset(&p, 0, sizeof p);
+    memset(&pi, 0, sizeof pi);
+    p.comp_count = comp_count;
+    p.interleaved = il;
+    p.color_space_internal = GPUJPEG_YCBCR_BT601_256LVLS;
+    for ( int c = 0; c < comp_count; c++ ) {
+        p.sampling_factor[c].horizontal = (uint8_t)hs[c];
+        p.sampling_factor[c].vertical = (uint8_t)vs[c];
+    }
+    pi.width = w;
+    pi.height = h;
+    pi.pixel_format = GPUJPEG_U8;
+    gj_geometry_init(g, &p, &pi);
+}
+
+int gj_transcode_plan(int w, int h, int comp_count, const int* hs_in, const int* vs_in, int src_interleaved, int out_interleaved, int rot,
+                      int flip, int perfect, struct gj_transcode_plan* pl, char* why)
+{
+    memset(pl, 0, sizeof *pl);
+    struct gj_orient_map m;
+    int ow, oh, src[4];
+    if ( w < 1 || h < 1 || comp_count < 1 || comp_count > GJ_MAX_COMP || gj_orient_frame(w, h, rot, flip, NULL, &ow, &oh, &m, src) ) {
+        snprintf(why, GJ_WHY_BYTES, "invalid frame (%dx%d, %d components)", w, h, comp_count);
+        return -1;
+    }
+    int hs[GJ_MAX_COMP], vs[GJ_MAX_COMP], max_h = 1, max_v = 1;
+    for ( int c = 0; c < comp_count; c++ ) {
+        hs[c] = comp_count == 1 ? 1 : hs_in[c];   /* a single component is never subsampled (T.81 A.2.2) */
+        vs[c] = comp_count == 1 ? 1 : vs_in[c];
+        if ( hs[c] > max_h ) max_h = hs[c];
+        if ( vs[c] > max_v ) max_v = vs[c];
+    }
+    /* a reversed source axis starts at the far edge: only whole iMCUs can move there */
+    const int imcu_w = 8 * max_h, imcu_h = 8 * max_v;
+    pl->neg_x = m.sxx < 0 || m.sxy < 0;
+    pl->neg_y = m.syx < 0 || m.syy < 0;
+    pl->transpose = m.sxx == 0;
+    const int tw = pl->neg_x ? w / imcu_w * imcu_w : w, th = pl->neg_y ? h / imcu_h * imcu_h : h;
+    if ( tw == 0 || th == 0 ) {
+        snprintf(why, GJ_WHY_BYTES, "a %dx%d frame has no whole %dx%d iMCU to turn or mirror", w, h, imcu_w, imcu_h);
+        return -1;
+    }
+    if ( perfect && (tw != w || th != h) ) {
+        snprintf(why, GJ_WHY_BYTES, "the %dx%d frame has partial %dx%d iMCUs at an edge that would move (perfect)", w, h, imcu_w, imcu_h);
+        return -1;
+    }
+    pl->src_w = tw;
+    pl->src_h = th;
+    pl->width = pl->transpose ? th : tw;
+    pl->height = pl->transpose ? tw : th;
+    for ( int c = 0; c < comp_count; c++ ) {
+        pl->hs[c] = pl->transpose ? vs[c] : hs[c];
+        pl->vs[c] = pl->transpose ? hs[c] : vs[c];
+    }
+    struct gj_geometry gs, gt, go;
+    plan_geometry(&gs, w, h, comp_count, hs, vs, src_interleaved);
+    plan_geometry(&gt, tw, th, comp_count, hs, vs, 0);   /* the trimmed planes' own blocks: the far edge of a reversed axis */
+    plan_geometry(&go, pl->width, pl->height, comp_count, pl->hs, pl->vs, out_interleaved);
+    for ( int c = 0; c < comp_count; c++ ) {
+        struct gj_blk_map* b = &pl->blk[c];
+        const int nbx = gt.comp[c].bcx, nby = gt.comp[c].bcy;
+        b->axx = m.sxx;
+        b->axy = m.sxy;
+        b->ayx = m.syx;
+        b->ayy = m.syy;
+        b->ax0 = pl->neg_x ? nbx - 1 : 0;
+        b->ay0 = pl->neg_y ? nby - 1 : 0;
+        b->src_bcx = gs.comp[c].bcx;
+        b->src_bcy = gs.comp[c].bcy;
+        b->out_bcx = go.comp[c].bcx;
+        b->out_bcy = go.comp[c].bcy;
+        const int lim_x = pl->neg_x ? nbx : b->src_bcx, lim_y = pl->neg_y ? nby : b->src_bcy;   /* source blocks along x / y */
+        const int lim_ox = pl->transpose ? lim_y : lim_x, lim_oy = pl->transpose ? lim_x : lim_y;
+        b->vis_bx = lim_ox < b->out_bcx ? lim_ox : b->out_bcx;
+        b->vis_by = lim_oy < b->out_bcy ? lim_oy : b->out_bcy;
+    }
+    return 0;
+}
+
+size_t gj_com_segments(const uint8_t* d, size_t size, uint8_t* out)
+{
+    size_t pos = 2, n = 0;
+    while ( pos + 4 <= size && d[pos] == 0xFF ) {
+        const int m = d[pos + 1];
+        if ( m == 0xFF ) {   /* fill byte */
+            pos++;
+            continue;
+        }
+        if ( m == 0xDA || m == 0xD9 ) break;
+        if ( m == 0xD8 || m == 0x01 || (m >= 0xD0 && m <= 0xD7) ) {   /* no length field */
+            pos += 2;
+            continue;
+        }
+        const size_t len = (size_t)((d[pos + 2] << 8) | d[pos + 3]);
+        if ( len < 2 || pos + 2 + len > size ) break;
+        if ( m == 0xFE ) {
+            if ( out ) memcpy(out + n, d + pos, 2 + len);
+            n += 2 + len;
+        }
+        pos += 2 + len;
+    }
+    return n;
+}
+
 int gj_crop_pick_units(int units_x, int units, int seg_units, int bpm, int ux0, int uy0, int ux1, int uy1, int seg_base,
                        uint32_t* out)
 {
@@ -435,15 +543,17 @@ size_t gj_write_header(uint8_t* out, const struct gpujpeg_parameters* param,
         p = w8(p, 0);
         p = w8(p, 0);
     }
+    /* quantisation tables: one per class, or the caller's per component (one DQT per table id, in the order of first use) */
+    const int own_q = extras && extras->comp_q;
     unsigned emitted = 0;
     for ( int c = 0; c < param->comp_count; c++ ) {
-        const int t = comp_is_luma(param, c) ? 0 : 1;
+        const int t = own_q ? extras->comp_tq[c] : comp_is_luma(param, c) ? 0 : 1;
         if ( emitted & (1u << t) ) continue;
         emitted |= 1u << t;
         p = wmark(p, 0xDB);
         p = w16(p, 67);
         p = w8(p, t);
-        memcpy(p, raw_q[t], 64);
+        memcpy(p, own_q ? extras->comp_q[c] : raw_q[t], 64);
         p += 64;
     }
     p = wmark(p, 0xC0);
@@ -455,7 +565,7 @@ size_t gj_write_header(uint8_t* out, const struct gpujpeg_parameters* param,
     for ( int c = 0; c < param->comp_count; c++ ) {
         p = w8(p, comp_id(param, c));
         p = w8(p, (param->sampling_factor[c].horizontal << 4) + param->sampling_factor[c].vertical);
-        p = w8(p, comp_is_luma(param, c) ? 0 : 1);
+        p = w8(p, own_q ? extras->comp_tq[c] : comp_is_luma(param, c) ? 0 : 1);
     }
     emitted = 0;
     for ( int c = 0; c < param->comp_count; c++ ) {
@@ -476,6 +586,10 @@ size_t gj_write_header(uint8_t* out, const struct gpujpeg_parameters* param,
     p = wmark(p, 0xDD);
     p = w16(p, 4);
     p = w16(p, param->restart_interval);
+    if ( extras && extras->com ) {
+        memcpy(p, extras->com, extras->com_size);
+        return (size_t)(p - out) + extras->com_size;
+    }
     char com[48];
     const int q = param->quality < 1 ? 1 : param->quality > 100 ? 100 : param->quality;
     const int n = snprintf(com, sizeof com, "CREATOR: GPUJPEG, quality = %d", q);

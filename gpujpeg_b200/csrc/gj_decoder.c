@@ -125,6 +125,13 @@ struct gpujpeg_decoder {
     struct gj_prog_scan* prog_scans;   /* [GJ_MAX_SCANS] */
     struct gj_dec_lut* h_prog_luts;    /* [GJ_MAX_SCANS * GJ_MAX_COMP] */
     struct gj_dec_lut* d_prog_luts;
+
+    /* gj_decoder_decode_coefficients: the frame stops after the Huffman stage with raw coefficients (no K4, no output); what
+     * it hands out besides the device buffers */
+    int coef_only;
+    uint8_t coef_qt[GJ_MAX_COMP][64];
+    int coef_tq[GJ_MAX_COMP];
+    uint8_t* com; size_t com_cap;
 };
 
 /* ---- output descriptor helpers [ref: src/gpujpeg_decoder.c:44-92] ---- */
@@ -222,6 +229,7 @@ int gpujpeg_decoder_destroy(struct gpujpeg_decoder* d)
     gj_cuda_free(d->d_prog_luts);
     gj_cuda_free(d->d_pick);
     gj_cuda_free(d->d_ss_scratch);
+    free(d->com);
     free(d->h_pick);
     free(d->prog_scans);
     free(d->h_prog_luts);
@@ -303,7 +311,7 @@ int gpujpeg_decoder_init(struct gpujpeg_decoder* d, const struct gpujpeg_paramet
     /* (the output of a scaled frame is smaller: gpujpeg_decoder_decode sizes d_raw for it, size_output) */
     if ( grow_dev((void**)&d->d_coef, &d->d_coef_size, g->coef_count * 2) ||
          grow_dev((void**)&d->d_cext, &d->d_cext_size, g->coef_count / 64) ||
-         (d->scale == 1 && grow_dev((void**)&d->d_raw, &d->d_raw_size, g->raw_size)) ) {
+         (d->scale == 1 && !d->coef_only && grow_dev((void**)&d->d_raw, &d->d_raw_size, g->raw_size)) ) {
         GJ_ERR("Decoder device allocation failed: %s\n", gj_cuda_last_error());
         return -1;
     }
@@ -1024,7 +1032,7 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
         pg.width = st->width;
         pg.height = st->height;
         p->interleaved = il;
-        if ( gpujpeg_decoder_init(d, p, &pg) || size_output(d, pi) ) return GPUJPEG_ERROR;
+        if ( gpujpeg_decoder_init(d, p, &pg) || (!d->coef_only && size_output(d, pi)) ) return GPUJPEG_ERROR;
     }
     const struct gj_geometry* g = &d->geo;
 
@@ -1064,6 +1072,11 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
         const uint8_t* q = st->have_comp_qt[c] ? st->comp_qt[c] : st->have_qt[st->comp_tq[c]] ? st->qt[st->comp_tq[c]] : NULL;
         for ( int k = 0; q && k < 64; k++ )
             d->h_tab.qinv_zz[c][k] = q[k];
+        if ( d->coef_only ) {
+            d->coef_tq[c] = st->comp_tq[c];
+            memset(d->coef_qt[c], 0, 64);
+            if ( q ) memcpy(d->coef_qt[c], q, 64);
+        }
     }
     const double t_reader_ms = (gpujpeg_get_time() - t_begin) * 1000.0;
     if ( !d->tab_valid || memcmp(&d->h_tab, &d->h_tab_prev, sizeof d->h_tab) != 0 ) {
@@ -1104,7 +1117,7 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
     a->d_coef = d->d_coef;
     a->d_cext = d->d_cext;
     a->coef_count = g->coef_count;
-    a->dequantize = d->idct_flavour == 0 && d->scale == 1;   /* the reduced IDCT dequantises the raw values itself */
+    a->dequantize = d->idct_flavour == 0 && d->scale == 1 && !d->coef_only;   /* the reduced IDCT dequantises the raw values itself */
     a->comp_count = g->comp_count;
     for ( int c = 0; c < g->comp_count; c++ )
         a->comp_blk_off[c] = g->comp[c].blk_off;
@@ -1127,8 +1140,8 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
         gj_timer_start(&d->t_dct, d->stream);
     }
     const int to_host = output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER || output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_BUFFER;
-    const int striped = to_host && !stats && stripes_usable(d);
-    if ( k4_and_output(d, output, pi, comp_tq, a->dequantize, striped, NULL, stats) ) return GPUJPEG_ERROR;
+    const int striped = to_host && !stats && !d->coef_only && stripes_usable(d);
+    if ( !d->coef_only && k4_and_output(d, output, pi, comp_tq, a->dequantize, striped, NULL, stats) ) return GPUJPEG_ERROR;
     if ( gj_cuda_memcpy_d2h_async(d->h_mk, d->d_mk, 16, d->stream) || gj_cuda_stream_sync(d->stream) ) {
         GJ_ERR("Decoder failed: %s\n", gj_cuda_last_error());
         return GPUJPEG_ERROR;
@@ -1308,7 +1321,8 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     }
     d->out_mode = out_mode;
     d->param_image.color_space = pi.color_space;
-    if ( ((out_mode != GJ_OUT_RGB || d->crop) && gj_raw_layout_init(&d->raw, &pi)) || size_output(d, &pi) ) return GPUJPEG_ERROR;
+    if ( !d->coef_only && (((out_mode != GJ_OUT_RGB || d->crop) && gj_raw_layout_init(&d->raw, &pi)) || size_output(d, &pi)) )
+        return GPUJPEG_ERROR;
     const struct gj_geometry* g = &d->geo;
 
     if ( st.progressive ) return decode_progressive(d, image, image_size, output, &st, &p, &pi, pos, adobe, early_cs, stats, t_begin);
@@ -1349,6 +1363,10 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         if ( !st.have_qt[st.comp_tq[c]] ) {
             GJ_ERR("Quantization table %d is missing!\n", st.comp_tq[c]);
             return GPUJPEG_ERROR;
+        }
+        if ( d->coef_only ) {
+            d->coef_tq[c] = st.comp_tq[c];
+            memcpy(d->coef_qt[c], st.qt[st.comp_tq[c]], 64);
         }
     }
 
@@ -1432,7 +1450,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     /* ---- K3 ---- */
     ha.d_file = d->d_file;
     ha.file_size = image_size;
-    ha.dequantize = d->idct_flavour == 0 && d->scale == 1;   /* the reduced IDCT dequantises the raw values itself */
+    ha.dequantize = d->idct_flavour == 0 && d->scale == 1 && !d->coef_only;   /* the reduced IDCT dequantises the raw values itself */
     ha.d_seg_off = by_table ? d->d_seg_off : NULL; /* segment starts: the stream's own table, or the device-built marker list */
     ha.d_seg_len = NULL;
     ha.d_list_pos = d->d_list_pos;
@@ -1512,7 +1530,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     /* host output of a large frame leaves stripe by stripe (decode_striped): K4 per stripe and, where the Huffman decoder can
      * work on a part of the frame, K3 per stripe as well -- the segments the stripe's rows need, just before its K4 */
     const int to_host = output->type == GPUJPEG_DECODER_OUTPUT_INTERNAL_BUFFER || output->type == GPUJPEG_DECODER_OUTPUT_CUSTOM_BUFFER;
-    const int striped = to_host && !stats && stripes_usable(d);
+    const int striped = to_host && !stats && !d->coef_only && stripes_usable(d);
     if ( d->k3_parts < 0 ) {
         const char* v = getenv("GPUJPEG_B200_STRIPES_K3");
         d->k3_parts = !(v && v[0] == '0');
@@ -1532,7 +1550,8 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         gj_timer_start(&d->t_dct, d->stream);
     }
 
-    if ( k4_and_output(d, output, &pi, st.comp_tq, ha.dequantize, striped, k3_striped ? &ha : NULL, stats) ) return GPUJPEG_ERROR;
+    if ( !d->coef_only && k4_and_output(d, output, &pi, st.comp_tq, ha.dequantize, striped, k3_striped ? &ha : NULL, stats) )
+        return GPUJPEG_ERROR;
     if ( gj_cuda_memcpy_d2h_async(d->h_mk, d->d_mk, 16, d->stream) || gj_cuda_stream_sync(d->stream) ) {
         GJ_ERR("Decoder failed: %s\n", gj_cuda_last_error());
         return GPUJPEG_ERROR;
@@ -1557,6 +1576,37 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
 
     record_stats(d, output, &pi, stats, t_reader_ms, t_begin);
     return GPUJPEG_NOERR;
+}
+
+int gj_decoder_decode_coefficients(struct gpujpeg_decoder* d, const uint8_t* image, size_t image_size, struct gj_coef_frame* f)
+{
+    if ( !d || !image || !f ) return -1;
+    struct gpujpeg_decoder_output output;
+    gpujpeg_decoder_output_set_default(&output);
+    d->coef_only = 1;
+    const int rc = gpujpeg_decoder_decode(d, (uint8_t*)image, image_size, &output);
+    d->coef_only = 0;
+    d->last_valid = 0;   /* a resident re-run would take the raw coefficients for K4's */
+    if ( rc ) return -1;
+    const size_t com = gj_com_segments(image, image_size, NULL);
+    if ( com > d->com_cap ) {
+        free(d->com);
+        d->com_cap = 0;
+        if ( !(d->com = (uint8_t*)malloc(com)) ) return -1;
+        d->com_cap = com;
+    }
+    memset(f, 0, sizeof *f);
+    f->geo = &d->geo;
+    f->d_coef = d->d_coef;
+    f->d_cext = d->d_cext;
+    f->progressive = d->last_progressive;
+    f->color_space = d->param.color_space_internal;
+    memcpy(f->qt, d->coef_qt, sizeof f->qt);
+    memcpy(f->tq, d->coef_tq, sizeof f->tq);
+    f->metadata = d->metadata;
+    f->com_size = gj_com_segments(image, image_size, d->com);
+    f->com = d->com;
+    return 0;
 }
 
 int gpujpeg_decoder_get_stats(struct gpujpeg_decoder* decoder, struct gpujpeg_duration_stats* stats)

@@ -59,6 +59,18 @@ GJ_HD constexpr int gj_nat2zz(int n)
     return t[n];
 }
 
+/* The transcoder's lossless turn / mirror of one block (k_coef_transform): zig-zag coefficient k of the output block is
+ * sign * coefficient gj_coef_src(k, ...) of the source block.  In natural order, v vertical and u horizontal frequency, the output's
+ * O[v][u] is S[u][v] under a transpose (output x runs along source y) and S[v][u] otherwise; a reversed source axis negates the
+ * source's odd frequencies along it, as a mirrored cosine basis function of odd frequency is the negated one. */
+GJ_HD int gj_coef_src(int k, int transpose, int neg_x, int neg_y, int* negate)
+{
+    const int n = gj_zz2nat(k), v = n >> 3, u = n & 7;
+    const int sv = transpose ? u : v, su = transpose ? v : u;
+    *negate = ((neg_x & su) ^ (neg_y & sv)) & 1;
+    return gj_nat2zz(sv * 8 + su);
+}
+
 /* ------------------------------------------------------------------------------------------- */
 /* block extents between K3 and K4 (format: GJ_CEXT_FULL in gj_internal.h)                       */
 

@@ -206,12 +206,46 @@ int gj_parse_orientation(const char* val, int* mode, int* rot, int* flip);
  * Returns -1 (and leaves the outputs alone) if crop does not lie inside the oriented image. */
 int gj_orient_frame(int w, int h, int rot, int flip, const int* crop, int* ow, int* oh, struct gj_orient_map* m, int src[4]);
 
+/* The transcoder's lossless turn / mirror (gj_transcoder.c, k_coef_transform).  Output block (bx, by) of component c shows the
+ * source block (sx, sy) = (axx * bx + axy * by + ax0, ayx * bx + ayy * by + ay0) of the same component when that lies in the
+ * source's src_bcx x src_bcy block grid of c; otherwise it is a dummy block, whose DC is that of the output block
+ * (min(bx, vis_bx - 1), min(by, vis_by - 1)) and whose AC coefficients are zero.  Coefficient signs and the transpose follow
+ * gj_coef_src (gj_device.cuh): transpose = output x runs along source y, neg_x / neg_y = the source's x / y axis is reversed. */
+struct gj_blk_map {
+    int axx, axy, ax0, ayx, ayy, ay0;
+    int src_bcx, src_bcy;              /* the source's block grid of the component */
+    int out_bcx, out_bcy;              /* the output's */
+    int vis_bx, vis_by;                /* output blocks [0, vis_bx) x [0, vis_by) show source blocks */
+};
+struct gj_transcode_plan {
+    int width, height;                 /* the output */
+    int hs[GJ_MAX_COMP], vs[GJ_MAX_COMP];
+    int transpose, neg_x, neg_y;
+    int src_w, src_h;                  /* the source after the trim */
+    struct gj_blk_map blk[GJ_MAX_COMP];
+};
+/* A w x h source of comp_count components with sampling hs / vs, its block grids those of gj_geometry_init (interleaved or not),
+ * turned rot quarter turns clockwise, then mirrored horizontally if flip, into an output of the same interleaving flag
+ * out_interleaved.  Without perfect, partial edge iMCUs that would move are dropped; with it such a frame is refused, as is a
+ * frame trimmed to nothing.  Returns 0, or -1 with the reason in why (GJ_WHY_BYTES). */
+#define GJ_WHY_BYTES 160
+int gj_transcode_plan(int w, int h, int comp_count, const int* hs, const int* vs, int src_interleaved, int out_interleaved, int rot,
+                      int flip, int perfect, struct gj_transcode_plan* plan, char* why);
+/* the COM segments of a JPEG file in front of its first SOS, markers included, copied to out (NULL: size only); their size */
+size_t gj_com_segments(const uint8_t* data, size_t size, uint8_t* out);
+
 /* ---- codestream writer (gj_writer.c)  [ref: src/gpujpeg_writer.c] ---- */
 /* what a header may carry besides the coding parameters: orientation (SPIFF directory entry / Exif tag) and user Exif tags */
 struct gj_exif_tags;
 struct gj_header_extras {
     struct gpujpeg_image_metadata metadata;
     const struct gj_exif_tags* exif_tags;
+    /* the transcoder: component c's quantisation table (zig-zag) and its table id, in place of raw_q by class (NULL: raw_q) */
+    const uint8_t (*comp_q)[64];
+    const uint8_t* comp_tq;
+    /* whole COM segments (markers included) that replace the writer's own comments; NULL: the writer's */
+    const uint8_t* com;
+    size_t com_size;
 };
 #define GJ_HEADER_BASE_CAP 1024   /* bytes a header needs at most without user Exif tags */
 size_t gj_write_header(uint8_t* out, const struct gpujpeg_parameters* param,
@@ -588,6 +622,50 @@ int gj_parse_bool(const char* val, const char* optname);
 /* the planes above described as a raw layout, so that the sample kernels can run on them (n samples per block side) */
 void gj_planes_layout(struct gj_raw_layout* l, struct gj_comp_geo padded[GJ_MAX_COMP], const struct gj_comp_geo* comp,
                       int comp_count, int n);
+
+/* The transcoder (gj_transcode.cu): the decoder's raw coefficients and block extents -> the encoder's coefficient buffer and
+ * non-zero masks, every output block through the plan's block map and coefficient map (the identity included).  *d_range is
+ * set non-zero when an output coefficient leaves the 8-bit baseline range (DC [-1024, 1023], AC [-1023, 1023]). */
+struct gj_coef_transform_args {
+    const int16_t* d_src;
+    const uint8_t* d_cext;
+    int src_blk_off[GJ_MAX_COMP];
+    int16_t* d_dst;
+    uint64_t* d_nzmask;
+    int dst_blk_off[GJ_MAX_COMP];
+    int comp_count;
+    int dst_blocks;
+    int transpose, neg_x, neg_y;
+    struct gj_blk_map blk[GJ_MAX_COMP];
+    uint32_t* d_range;
+};
+int gj_launch_coef_transform(const struct gj_coef_transform_args* a, gj_stream_t stream);
+
+/* The decoder up to its raw quantised coefficients (gj_decoder.c): every stream gpujpeg_decoder_decode takes, no IDCT, no output.
+ * The pointers stay valid until the decoder's next call. */
+struct gj_coef_frame {
+    const struct gj_geometry* geo;    /* block grids and their offsets in d_coef */
+    const int16_t* d_coef;            /* zig-zag, not dequantised */
+    const uint8_t* d_cext;
+    int progressive;
+    enum gpujpeg_color_space color_space;
+    uint8_t qt[GJ_MAX_COMP][64];      /* component c's quantisation table (zig-zag) and its table id */
+    int tq[GJ_MAX_COMP];
+    struct gpujpeg_image_metadata metadata;
+    const uint8_t* com;               /* the COM segments in front of the first SOS, markers included */
+    size_t com_size;
+};
+int gj_decoder_decode_coefficients(struct gpujpeg_decoder* d, const uint8_t* image, size_t image_size, struct gj_coef_frame* f);
+
+/* The encoder from coefficients (gj_encoder.c): gj_encoder_setup_coefficients sizes the encoder for a frame of parameters p
+ * (RESTART_AUTO as gpujpeg_encoder_encode resolves it for the frame, no segment info) and width x height with the header composed from comp_q / comp_tq, the COM
+ * segments com (replacing the writer's comments) and the metadata, and hands out where the coefficients and non-zero masks go
+ * (comp-major zig-zag blocks of *geo).  gj_encoder_finish runs what follows K1 in gpujpeg_encoder_encode. */
+int gj_encoder_setup_coefficients(struct gpujpeg_encoder* e, const struct gpujpeg_parameters* p, int width, int height,
+                                  const uint8_t comp_q[GJ_MAX_COMP][64], const uint8_t comp_tq[GJ_MAX_COMP], const uint8_t* com,
+                                  size_t com_size, const struct gpujpeg_image_metadata* metadata, int16_t** d_coef,
+                                  uint64_t** d_nzmask, const struct gj_geometry** geo);
+int gj_encoder_finish(struct gpujpeg_encoder* e, uint8_t** out, size_t* out_size);
 
 /* debug/test helper: device coefficient buffer (zig-zag) -> host natural order, block-major; coefficients past a block's
  * extent read as zero (d_cext NULL: every block is whole, as the encoder's) */

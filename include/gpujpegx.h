@@ -3,6 +3,8 @@
  * every name carries the prefix gpujpegx_).  The reference API itself is in libgpujpeg/gpujpeg.h.
  *
  *   * resident re-runs and coefficient read-back: used by bench.py and the parity tests
+ *   * gpujpegx_transcode*: lossless JPEG-to-JPEG rewrite (restart markers, fitted Huffman tables, baseline from progressive,
+ *     lossless turns and mirrors)
  *   * gpujpegx_batch_*: a batch of independent frames sharded over the GPUs of one box (SURVEY.md section 8e,
  *     BASELINE.json config 5).  The reference's only multi-device affordances are gpujpeg_init_device /
  *     gpujpeg_set_device (src/gpujpeg_common.c:219-288) and "one coder per host thread with its own stream"
@@ -48,6 +50,36 @@ GPUJPEG_API int gpujpegx_decoder_used_subsequences(const struct gpujpeg_decoder*
 /* measurement aid: rounds the sub-sequence kernel needed to reach its fixed point on the last frame (or on its last resident
  * re-run); 129 when it finished a segment in one thread.  Waits for the decoder's stream.  -1 if the frame did not run it */
 GPUJPEG_API int gpujpegx_decoder_subsequence_rounds(struct gpujpeg_decoder* decoder);
+
+/* ---- lossless JPEG-to-JPEG rewrite (what jpegtran -restart N -optimize -trim / -perfect does on a CPU) ----
+ * Every stream gpujpeg_decoder_decode takes (baseline with or without restart markers, progressive, 1, 3 or 4 components) is
+ * rewritten as one baseline frame with its quantised coefficients unchanged: the source's quantisation tables and COM
+ * segments, its interleaving (a progressive frame of several components becomes one interleaved scan), the restart interval
+ * and Huffman tables asked for, optionally turned and mirrored in the DCT domain.  One device and one stream per instance, not
+ * thread-safe per instance; a refused frame leaves the instance usable. */
+struct gpujpegx_transcoder;
+
+/* "none" (default), "auto" (the stream's SPIFF / Exif orientation) or "<deg>[-]" (deg 0, 90, 180, 270): turn clockwise, then
+ * mirror horizontally -- the grammar of dec_opt_orientation.  jpegtran's -flip horizontal = "0-", -flip vertical = "180-",
+ * -transpose = "90-", -transverse = "270-".  Orientation metadata is kept with "none" and dropped after any other transform. */
+#define GPUJPEGX_TRAN_OPT_TRANSFORM "tran_opt_transform"
+/* "0" (default): partial edge iMCUs that a transform would move are dropped (jpegtran -trim); "1": such a frame is refused
+ * (jpegtran -perfect) */
+#define GPUJPEGX_TRAN_OPT_PERFECT "tran_opt_perfect"
+/* "auto" (default: what RESTART_AUTO gives the encoder for the output's size, sampling and interleaving) or N >= 0 MCUs (0: no
+ * restart markers) */
+#define GPUJPEGX_TRAN_OPT_RESTART "tran_opt_restart"
+/* "standard" (default: T.81 Annex K tables) or "optimized" (tables fitted to the frame, as enc_opt_huffman=optimized) */
+#define GPUJPEGX_TRAN_OPT_HUFFMAN "tran_opt_huffman"
+
+/* NULL without a device */
+GPUJPEG_API struct gpujpegx_transcoder* gpujpegx_transcoder_create(cudaStream_t stream);
+GPUJPEG_API void gpujpegx_transcoder_destroy(struct gpujpegx_transcoder* t);
+/* 0 / -1 */
+GPUJPEG_API int gpujpegx_transcoder_set_option(struct gpujpegx_transcoder* t, const char* opt, const char* val);
+/* jpeg: host memory.  *out: transcoder-owned host buffer, valid until the next call or destroy.  0 / -1. */
+GPUJPEG_API int gpujpegx_transcode(struct gpujpegx_transcoder* t, const uint8_t* jpeg, size_t size, uint8_t** out,
+                                   size_t* out_size);
 
 /* ---- batches of independent frames over several GPUs ---- */
 struct gpujpegx_batch;
