@@ -300,13 +300,15 @@ class Encoder:
 class Decoder:
     """gpujpeg_decoder_create / gpujpeg_decoder_decode / gpujpeg_decoder_destroy"""
 
-    def __init__(self, stream=0, idct="int", scale="1", crop=None, huffman="auto", orientation="none"):
+    def __init__(self, stream=0, idct="int", scale="1", crop=None, huffman="auto", orientation="none", pixels="gpujpeg"):
         """scale: "1", "1/2", "1/4" or "1/8" -- decode to ceil(W * scale) x ceil(H * scale) pixels (dec_opt_scale)
         crop: (x, y, w, h) -- return only that rectangle of the (scaled, oriented) image (dec_opt_crop)
         huffman: "auto", "thread_per_segment" or "subsequence" -- the Huffman decoder kernel (dec_opt_huffman)
         orientation: "none", "auto" (the stream's SPIFF / Exif orientation) or "0" / "90" / "180" / "270", optionally followed
         by "-" -- turn the image clockwise, then mirror it horizontally (dec_opt_orientation); a quarter turn swaps the output's
-        width and height"""
+        width and height
+        pixels: "gpujpeg" or "libjpeg" -- the pixels libjpeg-turbo (PIL, torchvision) gives: ISLOW IDCT, fancy upsampling, its
+        YCbCr -> RGB (dec_opt_pixels); grey streams then decode to H x W (decode_samples)"""
         self._h = lib.gpujpeg_decoder_create(C.c_void_p(stream))
         if not self._h:
             raise GpuJpegError("gpujpeg_decoder_create failed (no CUDA device?)")
@@ -321,6 +323,8 @@ class Decoder:
             self.set_option("dec_opt_crop", "%dx%d+%d+%d" % (w, h, x, y))
         if orientation != "none":
             self.set_option("dec_opt_orientation", orientation)
+        if pixels != "gpujpeg":
+            self.set_option("dec_opt_pixels", pixels)
 
     def set_option(self, key, val):
         if lib.gpujpeg_decoder_set_option(self._h, key.encode(), val.encode()) != 0:

@@ -225,6 +225,17 @@ void gj_crop_blocks(const struct gj_geometry* g, int n, int x, int y, int w, int
     }
 }
 
+void gj_crop_widen(int width, int height, int max_hs, int max_vs, int r[4])
+{
+    const int x0 = r[0] - max_hs > 0 ? r[0] - max_hs : 0, y0 = r[1] - max_vs > 0 ? r[1] - max_vs : 0;
+    const int x1 = r[0] + r[2] + max_hs < width ? r[0] + r[2] + max_hs : width;
+    const int y1 = r[1] + r[3] + max_vs < height ? r[1] + r[3] + max_vs : height;
+    r[0] = x0;
+    r[1] = y0;
+    r[2] = x1 - x0;
+    r[3] = y1 - y0;
+}
+
 int gj_parse_orientation(const char* val, int* mode, int* rot, int* flip)
 {
     static const char* const deg[4] = {"0", "90", "180", "270"};

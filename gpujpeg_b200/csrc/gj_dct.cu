@@ -964,6 +964,7 @@ k_fdct_samples(const uint8_t* __restrict__ raw, const __grid_constant__ SampleGr
     quantise_store(v, prm.fwd_zz[g.table[comp]], coef + (size_t)bi * 64, nzmask + bi);
 }
 
+/* FLAVOUR as k_idct_rgb444, or GJ_IDCT_ISLOW (dec_opt_pixels=libjpeg, DEQ: raw coefficients) */
 template <int FLAVOUR, bool DEQ, bool WIN>
 __global__ void __launch_bounds__(SG_THREADS)
 k_idct_samples(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext, const __grid_constant__ SampleGrid g, int total_blocks,
@@ -998,6 +999,19 @@ k_idct_samples(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cex
 #pragma unroll
         for ( int i = 0; i < 16; i++ )
             px[i] = pack4_sat_u8(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+    }
+    else if ( FLAVOUR == GJ_IDCT_ISLOW ) {
+        /* dec_opt_pixels=libjpeg: jpeg_idct_islow on the raw coefficients, dequantised here in 32 bits (samples 0..255) */
+        int v[64];
+#pragma unroll
+        for ( int k = 0; k < 64; k++ ) {
+            const int c = (k & 1) ? (int)packed[k >> 1] >> 16 : (int)(short)(packed[k >> 1] & 0xFFFFu);
+            v[gj_zz2nat(k)] = (int)((uint32_t)c * (uint32_t)q[k]);
+        }
+        gj_idct_islow_block(v);
+#pragma unroll
+        for ( int i = 0; i < 16; i++ )
+            px[i] = (uint32_t)v[4 * i] | (uint32_t)v[4 * i + 1] << 8 | (uint32_t)v[4 * i + 2] << 16 | (uint32_t)v[4 * i + 3] << 24;
     }
     else {
         float f[64];
@@ -1091,6 +1105,68 @@ k_idct_scaled(const int16_t* __restrict__ coef, const uint8_t* __restrict__ cext
 #pragma unroll
         for ( int x = 0; x < N; x++ )
             if ( x < vw ) dst[(size_t)y * g.pitch[comp] + (size_t)x * g.xs[comp]] = (uint8_t)px[N * y + x];
+    }
+}
+
+/* dec_opt_pixels=libjpeg, the pass behind the ISLOW planes: every output pixel takes its source pixel through the orientation
+ * map (dec_opt_crop: the map starts at the rectangle's origin), luminance as it stands, every other component fancy-upsampled
+ * from its plane (gj_fancy_sample: ratios RH x RV, the real samples cw x ch), then libjpeg's colour conversion unless the stream
+ * is RGB-internal.  NC = 3 (RGB u8 interleaved) or 1 (grey).  A thread writes 4 pixels of an output row, as whole words where the
+ * row's bytes are 4-byte aligned. */
+struct LibjpegOut {
+    unsigned long long poff[3];
+    int ppitch[3];
+    int cw, ch;
+    int width, height;
+    unsigned long long pitch;
+    int rgb;
+    gj_orient_map m;
+};
+constexpr int LJ_THREADS = 128;
+
+template <int RH, int RV, int NC>
+__global__ void __launch_bounds__(LJ_THREADS)
+k_libjpeg_out(const uint8_t* __restrict__ planes, uint8_t* __restrict__ out, const __grid_constant__ LibjpegOut p)
+{
+    const int oy = blockIdx.y, ox0 = 4 * (blockIdx.x * LJ_THREADS + threadIdx.x);
+    if ( ox0 >= p.width ) return;
+    const gj_orient_map& m = p.m;
+    uint32_t o[NC];
+#pragma unroll
+    for ( int i = 0; i < NC; i++ )
+        o[i] = 0;
+#pragma unroll
+    for ( int j = 0; j < 4; j++ ) {
+        const int ox = min(ox0 + j, p.width - 1);   // (pixels past the row's end: any valid pixel, not stored)
+        const int sx = m.sxx * ox + m.sxy * oy + m.sx0, sy = m.syx * ox + m.syy * oy + m.sy0;
+        int c[3];
+        c[0] = __ldg(planes + p.poff[0] + (size_t)sy * p.ppitch[0] + sx);
+        if constexpr ( NC == 3 ) {
+#pragma unroll
+            for ( int k = 1; k < 3; k++ ) {
+                const uint8_t* pl = planes + p.poff[k];
+                const int pp = p.ppitch[k];
+                c[k] = gj_fancy_sample(sx, sy, RH, RV, p.cw, p.ch, [&](int cx, int cy) { return (int)__ldg(pl + (size_t)cy * pp + cx); });
+            }
+            if ( !p.rgb ) gj_ycc_rgb_libjpeg(c[0], c[1], c[2], c[0], c[1], c[2]);
+        }
+#pragma unroll
+        for ( int k = 0; k < NC; k++ ) {
+            const int b = NC * j + k;   // byte of the thread's group
+            o[b >> 2] |= (uint32_t)c[k] << (8 * (b & 3));
+        }
+    }
+    uint8_t* dst = out + (size_t)oy * p.pitch + (size_t)ox0 * NC;
+    if ( ox0 + 4 <= p.width && (reinterpret_cast<uintptr_t>(dst) & 3) == 0 ) {
+#pragma unroll
+        for ( int i = 0; i < NC; i++ )
+            reinterpret_cast<uint32_t*>(dst)[i] = o[i];
+    }
+    else {
+        const int nb = min(4, p.width - ox0) * NC;
+#pragma unroll
+        for ( int b = 0; b < 4 * NC; b++ )
+            if ( b < nb ) dst[b] = (uint8_t)(o[b >> 2] >> (8 * (b & 3)));
     }
 }
 
@@ -1484,6 +1560,7 @@ extern "C" int gj_launch_idct_samples(const int16_t* d_coef, const uint8_t* d_ce
     } while ( 0 )
     if ( idct_flavour == 0 && coef_dequantized ) GJ_K4S(0, false);
     else if ( idct_flavour == 0 ) GJ_K4S(0, true);
+    else if ( idct_flavour == GJ_IDCT_ISLOW ) GJ_K4S(GJ_IDCT_ISLOW, true);
     else GJ_K4S(1, true);
 #undef GJ_K4S
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
@@ -1513,5 +1590,34 @@ extern "C" int gj_launch_idct_scaled(const int16_t* d_coef, const uint8_t* d_cex
     else if ( n == 1 ) GJ_K4R(1);
     else return -1;
 #undef GJ_K4R
+    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+extern "C" int gj_launch_libjpeg_out(const uint8_t* d_planes, uint8_t* d_out, const struct gj_comp_geo* comp, int comp_count, int max_hs,
+                                     int max_vs, int width, int height, int rgb_internal, const struct gj_orient_map* map, gj_stream_t stream)
+{
+    if ( (comp_count != 1 && comp_count != 3) || width < 1 || height < 1 || !map ) return -1;
+    LibjpegOut p;
+    memset(&p, 0, sizeof p);
+    for ( int c = 0; c < comp_count; c++ ) {
+        p.poff[c] = (unsigned long long)comp[c].blk_off * 64;
+        p.ppitch[c] = comp[c].bcx * 8;
+    }
+    const int rh = comp_count == 3 ? max_hs / comp[1].hs : 1, rv = comp_count == 3 ? max_vs / comp[1].vs : 1;
+    if ( comp_count == 3 && (comp[0].hs != max_hs || comp[0].vs != max_vs || comp[1].hs != comp[2].hs || comp[1].vs != comp[2].vs) ) return -1;
+    p.cw = comp_count == 3 ? comp[1].width : 0;
+    p.ch = comp_count == 3 ? comp[1].height : 0;
+    p.width = width;
+    p.height = height;
+    p.pitch = (unsigned long long)width * comp_count;
+    p.rgb = rgb_internal;
+    p.m = *map;
+    const dim3 grid((width + 4 * LJ_THREADS - 1) / (4 * LJ_THREADS), height);
+    if ( comp_count == 1 ) k_libjpeg_out<1, 1, 1><<<grid, LJ_THREADS, 0, stream>>>(d_planes, d_out, p);
+    else if ( rh == 1 && rv == 1 ) k_libjpeg_out<1, 1, 3><<<grid, LJ_THREADS, 0, stream>>>(d_planes, d_out, p);
+    else if ( rh == 2 && rv == 1 ) k_libjpeg_out<2, 1, 3><<<grid, LJ_THREADS, 0, stream>>>(d_planes, d_out, p);
+    else if ( rh == 1 && rv == 2 ) k_libjpeg_out<1, 2, 3><<<grid, LJ_THREADS, 0, stream>>>(d_planes, d_out, p);
+    else if ( rh == 2 && rv == 2 ) k_libjpeg_out<2, 2, 3><<<grid, LJ_THREADS, 0, stream>>>(d_planes, d_out, p);
+    else return -1;
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -85,6 +85,8 @@ struct gpujpeg_decoder {
     int orient_mode, orient_rot, orient_flip;
     int orient;
     struct gj_orient_map omap;
+    /* dec_opt_pixels: pixels_req 1 = libjpeg (the option); a frame decoded that way runs with out_mode GJ_OUT_LIBJPEG */
+    int pixels_req;
     struct gpujpeg_image_metadata metadata;
 
     struct gj_dev_dec_tables h_tab, h_tab_prev;
@@ -336,8 +338,9 @@ void gpujpeg_decoder_set_output_format(struct gpujpeg_decoder* decoder, enum gpu
  *                   stream's sampling: 444-u8-p012, 444/422/420-u8-p0p1p2, 422-u8-p1020, or the special values
  *                   GPUJPEG_PIXFMT_NATIVE / _STD resolved as the reference does [ref: src/gpujpeg_reader.c:1507-1581]
  *   GJ_OUT_GENERIC  any of those pixel formats in GPUJPEG_RGB / _YCBCR_BT601 / _YCBCR_JPEG / _YCBCR_BT709 whatever the stream's
- *                   sampling: the IDCT writes component planes, one extra pass converts them (gj_convert.cu) */
-enum { GJ_OUT_RGB = 1, GJ_OUT_SAMPLES = 2, GJ_OUT_GENERIC = 3 };
+ *                   sampling: the IDCT writes component planes, one extra pass converts them (gj_convert.cu)
+ *   GJ_OUT_LIBJPEG  dec_opt_pixels=libjpeg (launch_k4_libjpeg): GPUJPEG_RGB 444-u8-p012 or GPUJPEG_U8, libjpeg-turbo's pixels */
+enum { GJ_OUT_RGB = 1, GJ_OUT_SAMPLES = 2, GJ_OUT_GENERIC = 3, GJ_OUT_LIBJPEG = 4 };
 
 static int choose_output(const struct gpujpeg_decoder* d, const struct gj_stream* st, struct gpujpeg_image_parameters* pi)
 {
@@ -450,10 +453,37 @@ static int launch_k4_crop(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_CO
                                  &d->omap, d->stream);
 }
 
+/* K4 of dec_opt_pixels=libjpeg, from the raw coefficients: jpeg_idct_islow (the ISLOW instances of the sample kernel) on the
+ * blocks of the frame -- of a cropped frame those of its rectangle widened by max_hs pixels and max_vs rows (gj_crop_widen), so
+ * that the upsampling has its neighbours --, then the pass that upsamples, converts, orients and crops (gj_launch_libjpeg_out).
+ * A grey frame as stored has nothing to upsample or convert: its ISLOW samples go straight into the output. */
+static int launch_k4_libjpeg(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], uint8_t* d_out)
+{
+    const struct gj_geometry* g = &d->geo;
+    struct gj_k4_window win;
+    memset(&win, 0, sizeof win);
+    memcpy(win.blk, d->crop_blk, sizeof win.blk);
+    if ( g->comp_count == 1 && !d->orient ) {
+        win.ox[0] = d->crop_x;
+        win.oy[0] = d->crop_y;
+        return gj_launch_idct_samples(d->d_coef, d->d_cext, d->scomp, 1, comp_tq, d_out, &d->raw, GJ_IDCT_ISLOW, 0, &d->h_tab,
+                                      d->crop ? &win : NULL, d->stream);
+    }
+    struct gj_raw_layout pl;
+    struct gj_comp_geo padded[GJ_MAX_COMP];
+    gj_planes_layout(&pl, padded, g->comp, g->comp_count, 8);
+    if ( gj_launch_idct_samples(d->d_coef, d->d_cext, padded, g->comp_count, comp_tq, d->d_planes, &pl, GJ_IDCT_ISLOW, 0, &d->h_tab,
+                                d->crop ? &win : NULL, d->stream) )
+        return -1;
+    return gj_launch_libjpeg_out(d->d_planes, d_out, g->comp, g->comp_count, g->max_hs, g->max_vs, d->out_w, d->out_h,
+                                 d->param.color_space_internal == GPUJPEG_RGB, &d->omap, d->stream);
+}
+
 /* K4 for the coder's geometry: the 4:4:4 kernel or the chroma-subsampling template instance */
 static int launch_k4(struct gpujpeg_decoder* d, const int comp_tq[GJ_MAX_COMP], uint8_t* d_out, int coef_dequantized)
 {
     const struct gj_geometry* g = &d->geo;
+    if ( d->out_mode == GJ_OUT_LIBJPEG ) return launch_k4_libjpeg(d, comp_tq, d_out);
     if ( d->crop ) return launch_k4_crop(d, comp_tq, d_out, coef_dequantized);
     if ( d->scale > 1 ) return launch_k4_scaled(d, comp_tq, d_out);
     if ( d->out_mode == GJ_OUT_SAMPLES )
@@ -968,11 +998,22 @@ static int size_output(struct gpujpeg_decoder* d, const struct gpujpeg_image_par
         d->scomp[c].height = (pi->height + div_v - 1) / div_v;
     }
     if ( grow_dev((void**)&d->d_raw, &d->d_raw_size, d->out_size) ||
-         (d->out_mode == GJ_OUT_GENERIC && grow_dev((void**)&d->d_planes, &d->d_planes_size, g->coef_count / 64 * n * n)) ) {
+         ((d->out_mode == GJ_OUT_GENERIC || d->out_mode == GJ_OUT_LIBJPEG) &&
+          grow_dev((void**)&d->d_planes, &d->d_planes_size, g->coef_count / 64 * n * n)) ) {
         GJ_ERR("Decoder device allocation failed: %s\n", gj_cuda_last_error());
         return -1;
     }
     return 0;
+}
+
+/* dec_opt_crop: the blocks of every component the frame's rectangle needs (d->crop_blk), for K4 and the segment pick; under
+ * dec_opt_pixels=libjpeg those of the rectangle widened for the upsampling's neighbours */
+static void crop_blocks(struct gpujpeg_decoder* d)
+{
+    const struct gj_geometry* g = &d->geo;
+    int r[4] = {d->crop_x, d->crop_y, d->crop_w, d->crop_h};
+    if ( d->out_mode == GJ_OUT_LIBJPEG ) gj_crop_widen(g->width, g->height, g->max_hs, g->max_vs, r);
+    gj_crop_blocks(g, 8 / d->scale, r[0], r[1], r[2], r[3], d->crop_blk);
 }
 
 /* dec_opt_crop: room for `pairs` {segment, blocks} pairs on the host and the device */
@@ -1093,7 +1134,7 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
         size_t pairs = 0;
         for ( int k = 0; k < st->scan_count; k++ )
             pairs += (size_t)d->prog_scans[k].seg_count;
-        gj_crop_blocks(g, 8 / d->scale, d->crop_x, d->crop_y, d->crop_w, d->crop_h, d->crop_blk);
+        crop_blocks(d);
         if ( grow_pick(d, pairs) ) {
             GJ_ERR("Decoder allocation failed: %s\n", gj_cuda_last_error());
             return GPUJPEG_ERROR;
@@ -1117,7 +1158,8 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
     a->d_coef = d->d_coef;
     a->d_cext = d->d_cext;
     a->coef_count = g->coef_count;
-    a->dequantize = d->idct_flavour == 0 && d->scale == 1 && !d->coef_only;   /* the reduced IDCT dequantises the raw values itself */
+    /* the reduced IDCT and ISLOW dequantise the raw values themselves */
+    a->dequantize = d->idct_flavour == 0 && d->scale == 1 && !d->coef_only && d->out_mode != GJ_OUT_LIBJPEG;
     a->comp_count = g->comp_count;
     for ( int c = 0; c < g->comp_count; c++ )
         a->comp_blk_off[c] = g->comp[c].blk_off;
@@ -1154,6 +1196,21 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
     output->metadata = &d->metadata;
     record_stats(d, output, pi, stats, t_reader_ms, t_begin);
     return GPUJPEG_NOERR;
+}
+
+/* dec_opt_pixels=libjpeg is defined for full-range YCbCr (JFIF, Adobe transform 1), RGB-internal (Adobe transform 0) and grey
+ * streams, at scale 1, with the default IDCT option, no flip and no channel remap: 1 (with a message) for anything else */
+static int libjpeg_refused(const struct gpujpeg_decoder* d, const struct gj_stream* st, enum gpujpeg_color_space cs)
+{
+    const char* why = st->comp_count == 4                                                        ? "4-component streams"
+                      : cs != GPUJPEG_YCBCR_BT601_256LVLS && cs != GPUJPEG_RGB                  ? gpujpeg_color_space_get_name(cs)
+                      : d->scale_req != 1                                                       ? GPUJPEG_DEC_OPT_SCALE " other than 1"
+                      : d->flipped                                                              ? GPUJPEG_DEC_OPT_FLIPPED_BOOL
+                      : d->channel_remap                                                        ? GPUJPEG_DEC_OPT_CHANNEL_REMAP
+                      : d->idct_flavour != 0                                                    ? GPUJPEG_DEC_OPT_IDCT " other than int"
+                                                                                                : NULL;
+    if ( why ) GJ_ERR("dec_opt_pixels=libjpeg is not supported for %s.\n", why);
+    return why != NULL;
 }
 
 /* [ref: src/gpujpeg_decoder.c:234-469] */
@@ -1242,6 +1299,9 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         GJ_ERR("dec_opt_flipped is not supported together with dec_opt_orientation.\n");
         return GPUJPEG_ERROR;
     }
+    /* dec_opt_pixels=libjpeg: the streams and options it is defined for */
+    const int libjpeg = d->pixels_req && !d->coef_only;
+    if ( libjpeg && libjpeg_refused(d, &st, early_cs) ) return GPUJPEG_ERROR;
     /* the frame's scale, rectangle and orientation are committed to the decoder only once nothing below can refuse the frame: a
      * refused frame leaves the last frame's state, which a resident re-run may still use, untouched */
     const int scale = d->scale_req;
@@ -1265,6 +1325,15 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     }
     int out_mode = choose_output(d, &st, &pi);
     if ( !out_mode ) return GPUJPEG_ERROR;
+    if ( libjpeg ) {
+        if ( st.comp_count == 3 ? pi.pixel_format != GPUJPEG_444_U8_P012 || pi.color_space != GPUJPEG_RGB
+                                : pi.color_space != GPUJPEG_YCBCR_BT601_256LVLS ) {
+            GJ_ERR("dec_opt_pixels=libjpeg produces GPUJPEG_RGB 444-u8-p012 (grey streams: GPUJPEG_U8) only (%s %s requested).\n",
+                   gpujpeg_color_space_get_name(pi.color_space), gpujpeg_pixel_format_get_name(pi.pixel_format));
+            return GPUJPEG_ERROR;
+        }
+        out_mode = GJ_OUT_LIBJPEG;
+    }
     /* the 2:1 chroma pairs of a turned or mirrored image of odd size are not the source's pairs turned */
     if ( orient && (pi.pixel_format == GPUJPEG_422_U8_P1020 || pi.pixel_format == GPUJPEG_422_U8_P0P1P2 ||
                     pi.pixel_format == GPUJPEG_420_U8_P0P1P2) ) {
@@ -1450,7 +1519,8 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     /* ---- K3 ---- */
     ha.d_file = d->d_file;
     ha.file_size = image_size;
-    ha.dequantize = d->idct_flavour == 0 && d->scale == 1 && !d->coef_only;   /* the reduced IDCT dequantises the raw values itself */
+    /* the reduced IDCT and ISLOW dequantise the raw values themselves */
+    ha.dequantize = d->idct_flavour == 0 && d->scale == 1 && !d->coef_only && d->out_mode != GJ_OUT_LIBJPEG;
     ha.d_seg_off = by_table ? d->d_seg_off : NULL; /* segment starts: the stream's own table, or the device-built marker list */
     ha.d_seg_len = NULL;
     ha.d_list_pos = d->d_list_pos;
@@ -1503,7 +1573,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     }
     /* a cropped frame: the blocks K4 transforms; K3 decodes the segments that hold them (gj_crop_pick), one thread per segment,
      * unless the sub-sequence kernel decodes the whole frame */
-    if ( d->crop ) gj_crop_blocks(g, 8 / d->scale, d->crop_x, d->crop_y, d->crop_w, d->crop_h, d->crop_blk);
+    if ( d->crop ) crop_blocks(d);
     if ( d->crop && !ha.subsequence ) {
         if ( grow_pick(d, (size_t)g->seg_count) ) {
             GJ_ERR("Decoder allocation failed: %s\n", gj_cuda_last_error());
@@ -1791,6 +1861,15 @@ int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt,
         decoder->orient_flip = flip;
         return GPUJPEG_NOERR;
     }
+    if ( strcmp(opt, GPUJPEG_DEC_OPT_PIXELS) == 0 ) {
+        if ( strcmp(val, GPUJPEG_DEC_PIXELS_VAL_GPUJPEG) == 0 ) decoder->pixels_req = 0;
+        else if ( strcmp(val, GPUJPEG_DEC_PIXELS_VAL_LIBJPEG) == 0 ) decoder->pixels_req = 1;
+        else {
+            GJ_ERR("Unknown output pixels: %s (gpujpeg or libjpeg)\n", val);
+            return GPUJPEG_ERROR;
+        }
+        return GPUJPEG_NOERR;
+    }
     if ( strcmp(opt, GPUJPEG_DEC_OPT_TGA_RLE_BOOL) == 0 || strcmp(opt, GPUJPEG_DEC_OPT_ALIGNMENT_BYTES_INT) == 0 ) {
         GJ_ERR("Decoder option %s is not implemented in this build.\n", opt);
         return GPUJPEG_ERROR;
@@ -1811,6 +1890,9 @@ void gpujpeg_decoder_print_options(void)
            "the restart segments it covers (default: none)\n");
     printf("\t" GPUJPEG_DEC_OPT_ORIENTATION "=[none|auto|<deg>[-]] - turn the output <deg> = 0, 90, 180 or 270 degrees clockwise, then "
            "mirror it horizontally with '-'; auto: as the stream's SPIFF or Exif orientation says (default: none)\n");
+    printf("\t" GPUJPEG_DEC_OPT_PIXELS "=[" GPUJPEG_DEC_PIXELS_VAL_GPUJPEG "|" GPUJPEG_DEC_PIXELS_VAL_LIBJPEG "] - the pixels of "
+           "gpujpeg's arithmetic, or those libjpeg-turbo's jpeg_read_scanlines returns with its default parameters: ISLOW IDCT, fancy "
+           "upsampling, its YCbCr -> RGB (default: gpujpeg)\n");
 }
 
 GPUJPEG_API int gpujpegx_decoder_used_segment_info(const struct gpujpeg_decoder* d)

@@ -504,6 +504,111 @@ GJ_HD void gj_idct_scaled_block(const int (&in)[64], int (&out)[N * N])
 }
 
 /* ------------------------------------------------------------------------------------------- */
+/* dec_opt_pixels=libjpeg: what libjpeg-turbo's jpeg_read_scanlines returns with its default decompression parameters        */
+/* (JDCT_ISLOW, do_fancy_upsampling, jdcolor's ycc_rgb_convert)                                                              */
+
+/* One 1-D pass of jidctint.c's jpeg_idct_islow (CONST_BITS 13, the twelve FIX_* constants): d[k] = input of frequency k,
+ * o[i] = DESCALE(output i, shift).  Every sum and product wraps in 32 bits, as in gj_idct_scaled_block. */
+GJ_HD void gj_islow1(const uint32_t (&d)[8], int shift, int (&o)[8])
+{
+    const uint32_t z1e = (d[2] + d[6]) * 4433u;
+    const uint32_t t2e = z1e - d[6] * 15137u, t3e = z1e + d[2] * 6270u;
+    const uint32_t t0e = (d[0] + d[4]) << 13, t1e = (d[0] - d[4]) << 13;
+    const uint32_t t10 = t0e + t3e, t13 = t0e - t3e, t11 = t1e + t2e, t12 = t1e - t2e;
+    uint32_t t0 = d[7], t1 = d[5], t2 = d[3], t3 = d[1];
+    uint32_t z1 = t0 + t3, z2 = t1 + t2, z3 = t0 + t2, z4 = t1 + t3;
+    const uint32_t z5 = (z3 + z4) * 9633u;
+    t0 *= 2446u;
+    t1 *= 16819u;
+    t2 *= 25172u;
+    t3 *= 12299u;
+    z1 *= (uint32_t)-7373;
+    z2 *= (uint32_t)-20995;
+    z3 = z3 * (uint32_t)-16069 + z5;
+    z4 = z4 * (uint32_t)-3196 + z5;
+    t0 += z1 + z3;
+    t1 += z2 + z4;
+    t2 += z2 + z3;
+    t3 += z1 + z4;
+    o[0] = gj_red_descale(t10 + t3, shift);
+    o[7] = gj_red_descale(t10 - t3, shift);
+    o[1] = gj_red_descale(t11 + t2, shift);
+    o[6] = gj_red_descale(t11 - t2, shift);
+    o[2] = gj_red_descale(t12 + t1, shift);
+    o[5] = gj_red_descale(t12 - t1, shift);
+    o[3] = gj_red_descale(t13 + t0, shift);
+    o[4] = gj_red_descale(t13 - t0, shift);
+}
+/* jpeg_idct_islow on one block, in place.  In: the RAW quantised coefficient times its quantiser as a 32-bit integer, natural
+ * order (not the int16-wrapped product of the integer flavour).  Columns first, descaled by CONST_BITS - PASS1_BITS = 11, then
+ * rows, descaled by CONST_BITS + PASS1_BITS + 3 = 18, through libjpeg's range limit.  Out: 64 samples 0..255, row-major.  The
+ * zero-column / zero-row shortcuts of jidctint.c give the full formulas' values wherever no intermediate leaves 31 bits and are
+ * left out; beyond that (hand-built blocks, never an 8-bit encoder's) the 32-bit wrap defines the result. */
+GJ_HD void gj_idct_islow_block(int (&v)[64])
+{
+#pragma unroll
+    for ( int c = 0; c < 8; c++ ) {
+        const uint32_t d[8] = {(uint32_t)v[c], (uint32_t)v[8 + c], (uint32_t)v[16 + c], (uint32_t)v[24 + c],
+                               (uint32_t)v[32 + c], (uint32_t)v[40 + c], (uint32_t)v[48 + c], (uint32_t)v[56 + c]};
+        int o[8];
+        gj_islow1(d, 11, o);
+#pragma unroll
+        for ( int r = 0; r < 8; r++ )
+            v[8 * r + c] = o[r];
+    }
+#pragma unroll
+    for ( int r = 0; r < 8; r++ ) {
+        const uint32_t d[8] = {(uint32_t)v[8 * r], (uint32_t)v[8 * r + 1], (uint32_t)v[8 * r + 2], (uint32_t)v[8 * r + 3],
+                               (uint32_t)v[8 * r + 4], (uint32_t)v[8 * r + 5], (uint32_t)v[8 * r + 6], (uint32_t)v[8 * r + 7]};
+        int o[8];
+        gj_islow1(d, 18, o);
+#pragma unroll
+        for ( int i = 0; i < 8; i++ )
+            v[8 * r + i] = gj_red_limit(o[i]);
+    }
+}
+
+/* Fancy upsampling as libjpeg-turbo's jinit_upsampler picks it, for the sample that output pixel (x, y) takes from a component
+ * with rh x rv times fewer samples (ratios against the largest sampling factors); cw x ch are its REAL samples,
+ * ceil(W * h / hmax) x ceil(H * v / vmax), and s(cx, cy) reads sample (cx, cy) of them.  Beyond the real samples the last one is
+ * replicated (jdmainct's context rows, the end columns of jdsample's loops):
+ *   2x1 h2v1_fancy_upsample : (3 c + left + 1) >> 2, (3 c + right + 2) >> 2
+ *   1x2 h1v2_fancy_upsample : (3 c + above + 1) >> 2, (3 c + below + 2) >> 2
+ *   2x2 h2v2_fancy_upsample : column sums s = 3 c + (row above | row below), then (3 s + left + 8) >> 4, (3 s + right + 7) >> 4
+ * 2x1 and 2x2 are fancy only for components of more than two samples per row; otherwise, and for every other ratio, the
+ * sample is replicated (h2v1_upsample, h2v2_upsample, int_upsample). */
+template <class S>
+GJ_HD int gj_fancy_sample(int x, int y, int rh, int rv, int cw, int ch, S s)
+{
+    const int cx = x / rh, cy = y / rv;
+    if ( rh == 2 && rv == 1 && cw > 2 ) {
+        const int nx = (x & 1) ? (cx + 1 < cw ? cx + 1 : cw - 1) : (cx > 0 ? cx - 1 : 0);
+        return (3 * s(cx, cy) + s(nx, cy) + 1 + (x & 1)) >> 2;
+    }
+    if ( rh == 1 && rv == 2 ) {
+        const int ny = (y & 1) ? (cy + 1 < ch ? cy + 1 : ch - 1) : (cy > 0 ? cy - 1 : 0);
+        return (3 * s(cx, cy) + s(cx, ny) + 1 + (y & 1)) >> 2;
+    }
+    if ( rh == 2 && rv == 2 && cw > 2 ) {
+        const int nx = (x & 1) ? (cx + 1 < cw ? cx + 1 : cw - 1) : (cx > 0 ? cx - 1 : 0);
+        const int ny = (y & 1) ? (cy + 1 < ch ? cy + 1 : ch - 1) : (cy > 0 ? cy - 1 : 0);
+        const int near = 3 * s(cx, cy) + s(cx, ny), far = 3 * s(nx, cy) + s(nx, ny);
+        return (3 * near + far + 8 - (x & 1)) >> 4;
+    }
+    return s(cx, cy);
+}
+
+/* jdcolor.c's ycc_rgb_convert (its tables spelled out, SCALEBITS 16, arithmetic shifts), clamped to 0..255 */
+GJ_HD void gj_ycc_rgb_libjpeg(int y, int cb, int cr, int& r, int& g, int& b)
+{
+    cb -= 128;
+    cr -= 128;
+    r = gj_clamp8(y + ((91881 * cr + 32768) >> 16));
+    g = gj_clamp8(y + ((-22554 * cb + 32768 - 46802 * cr) >> 16));
+    b = gj_clamp8(y + ((116130 * cb + 32768) >> 16));
+}
+
+/* ------------------------------------------------------------------------------------------- */
 /* Huffman helpers                                                                               */
 
 /* number of significant bits of |v| (JPEG "category")  [ref: src/gpujpeg_huffman_cpu_encoder.c:159-164] */

@@ -183,6 +183,10 @@ struct gj_blk_rect {
     int bx0, by0, bx1, by1;
 };
 void gj_crop_blocks(const struct gj_geometry* g, int n, int x, int y, int w, int h, struct gj_blk_rect win[GJ_MAX_COMP]);
+/* dec_opt_pixels=libjpeg: fancy upsampling reads one chroma sample on every side of the one under a pixel, so the blocks a
+ * rectangle needs are those of r = {x, y, w, h} widened by max_hs pixels and max_vs rows, clamped to the width x height image
+ * (in place) */
+void gj_crop_widen(int width, int height, int max_hs, int max_vs, int r[4]);
 /* The restart segments of a scan that hold a unit (MCU) of the rectangle [ux0, ux1) x [uy0, uy1) of its units_x-wide unit
  * grid, seg_units units per segment, bpm blocks per unit: pairs {seg_base + segment, blocks to decode} in ascending order,
  * the block count reaching up to and including the segment's last needed unit.  Returns the number of pairs. */
@@ -590,6 +594,14 @@ int gj_launch_idct_samples(const int16_t* d_coef, const uint8_t* d_cext, const s
                            const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int idct_flavour, int coef_dequantized,
                            const struct gj_dev_dec_tables* h_tables, const struct gj_k4_window* win /* NULL: every block */,
                            gj_stream_t stream);
+/* idct_flavour of gj_launch_idct_samples for dec_opt_pixels=libjpeg: libjpeg's jpeg_idct_islow (gj_idct_islow_block) on RAW
+ * coefficients (coef_dequantized 0) */
+#define GJ_IDCT_ISLOW 2
+/* dec_opt_pixels=libjpeg behind the ISLOW planes (gj_planes_layout, n = 8; comp = the stream's geometry, whose width / height are
+ * every component's real samples): the width x height output, RGB u8 interleaved (3 components) or grey u8, pixel (x, y) showing
+ * source pixel `map` (x, y) -- luminance, fancy-upsampled chroma (gj_fancy_sample), jdcolor's YCbCr -> RGB unless rgb_internal */
+int gj_launch_libjpeg_out(const uint8_t* d_planes, uint8_t* d_out, const struct gj_comp_geo* comp, int comp_count, int max_hs, int max_vs,
+                          int width, int height, int rgb_internal, const struct gj_orient_map* map, gj_stream_t stream);
 /* K4 of scaled decoding (dec_opt_scale): libjpeg's reduced inverse DCT, n = 4, 2 or 1 samples per block side (scale 1/2, 1/4,
  * 1/8), from RAW quantised coefficients; comp[c].width / height are the component's sample extents at that scale */
 int gj_launch_idct_scaled(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,

@@ -520,6 +520,21 @@ GPUJPEG_API int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size
  * gpujpeg_decoder_get_image_info2 still reports the stream as stored.  Refused for a frame it turns or mirrors: together with
  * dec_opt_flipped, and pixel formats with chroma subsampling (422-u8-p1020, 422-u8-p0p1p2, 420-u8-p0p1p2). */
 #define GPUJPEG_DEC_OPT_ORIENTATION "dec_opt_orientation"
+/* Extension of this build (not in the reference): which pixels the decoder returns.  "gpujpeg" (default): those of the
+ * reference's arithmetic (its integer IDCT, chroma replicated by sample, its colour formulas).  "libjpeg": the pixels
+ * libjpeg-turbo's jpeg_read_scanlines returns with its default decompression parameters -- what PIL's
+ * Image.open(...).convert("RGB") and torchvision's decode_jpeg give --: jidctint.c's JDCT_ISLOW on the raw quantised
+ * coefficients, fancy upsampling of subsampled chroma (jdsample.c's h2v1 / h1v2 / h2v2 triangle filters; replication for
+ * components of at most two samples per row at 2:1 horizontally), jdcolor.c's YCbCr -> RGB.  For streams read as full-range
+ * YCbCr (JFIF, Adobe transform 1), as RGB (Adobe transform 0, no colour conversion) or grey, baseline or progressive, every
+ * sampling the decoder takes, with dec_opt_crop (the uncropped output cut to the rectangle) and dec_opt_orientation.  Output:
+ * GPUJPEG_RGB 444-u8-p012, GPUJPEG_U8 for grey streams (the formats chosen when the caller sets none).  Refused with a
+ * message, the decoder staying usable: streams read as BT.601 limited range or BT.709 (SPIFF), 4-component streams, every
+ * other output format or colour space, dec_opt_scale other than 1, dec_opt_flipped, dec_opt_channel_remap, dec_opt_idct other
+ * than "int". */
+#define GPUJPEG_DEC_OPT_PIXELS "dec_opt_pixels"
+#define GPUJPEG_DEC_PIXELS_VAL_GPUJPEG "gpujpeg"
+#define GPUJPEG_DEC_PIXELS_VAL_LIBJPEG "libjpeg"
 GPUJPEG_API int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt, const char* val);
 GPUJPEG_API void gpujpeg_decoder_print_options(void);
 
