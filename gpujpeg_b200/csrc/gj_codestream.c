@@ -207,8 +207,10 @@ int gj_geometry_init(struct gj_geometry* g, const struct gpujpeg_parameters* par
     }
     /* worst case per 8x8 block: 64 x (16-bit code + 11 value bits) < 208 bytes, doubled by stuffing */
     g->slot_stride = ((size_t)g->seg_mcu * (g->interleaved ? l->bpm : 1) * 416 + 2 + 127) / 128 * 128;
-    /* same budget as the reference's output buffer [ref: src/gpujpeg_writer.c:63-89] */
-    g->stream_cap = 4096 + (size_t)pi->width * pi->height * g->comp_count * 2;
+    /* the reference's output budget [ref: src/gpujpeg_writer.c:63-89], 2 bytes per pixel and component -- or per coded
+     * sample where padding to whole blocks and MCUs outweighs the image: a frame 1 pixel thin codes 8 rows per real one */
+    const size_t samples = (size_t)pi->width * pi->height * g->comp_count;
+    g->stream_cap = 4096 + (g->coef_count > samples ? g->coef_count : samples) * 2;
     if ( param->segment_info ) g->stream_cap += ((size_t)g->seg_count + GJ_MAX_COMP) * 4 + 5 * ((size_t)g->seg_count * 4 / GJ_SEGINFO_CHUNK + 2 * GJ_MAX_COMP);
     return 0;
 }

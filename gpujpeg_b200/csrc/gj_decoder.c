@@ -1398,6 +1398,13 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
 
     /* ---- upload the file once, untouched; K0 builds the marker list on the device ---- */
     const size_t ecs_begin = st.scan[0].begin;
+    /* K0 tiles the file from a 16-byte aligned base below the first scan and its tile status holds 31-bit counts; a stream
+     * whose scans span 2^31 bytes or more is refused here, before any upload, whether or not it carries segment-info tables
+     * (which would skip K0), so that both forms of one stream get the same answer */
+    if ( image_size - (ecs_begin & ~(size_t)15) >= ((size_t)1 << 31) ) {
+        GJ_ERR("JPEG entropy-coded data of %zu bytes exceeds the supported maximum of 2^31 bytes.\n", image_size - ecs_begin);
+        return GPUJPEG_ERROR;
+    }
     const uint32_t list_cap = (uint32_t)g->seg_count + GJ_MK_OTHER_CAP;
     if ( upload_file(d, image, image_size, ecs_begin, list_cap, stats) ) return GPUJPEG_ERROR;
     uint32_t first_rank[GJ_MAX_COMP] = {0, 0, 0, 0}, end_rank[GJ_MAX_COMP] = {0, 0, 0, 0}, scan_cbegin[GJ_MAX_COMP] = {0, 0, 0, 0};
