@@ -455,6 +455,65 @@ int gj_crop_pick(const struct gj_geometry* g, int k, const struct gj_blk_rect wi
     return gj_crop_pick_units(units_x, l->scan_mcus[k], g->seg_mcu, l->bpm, ux0, uy0, ux1, uy1, l->scan_seg_begin[k], out);
 }
 
+/* The kernels were timed by frame size and content with profiles/k3_matrix.py on an H100 SXM.
+ * - Self-synchronising (gj_huffdec.cu), several lanes per restart segment: a frame with few segments cannot occupy the GPU
+ *   with one thread per segment, the walks buy parallelism INSIDE a segment (4K photo: 66 us against 102).  With 30 000
+ *   segments and more the segments alone keep the machine busy and the redundant walks pay off only for dense segments, 8 to
+ *   20 bytes per block (8K q90: 330 us with 32 lanes against 401), not at photographic q75 densities (8K: 205 against 212
+ *   with the best lane count), for very sparse or for random content.  Interleaved scans: a walk that starts inside the
+ *   stream also has to guess which component's block it is in, and a wrong guess does not heal by itself (other Huffman
+ *   tables) -- exactness then spreads one lane per round; one thread per segment is faster at every size.
+ * - Sub-sequences (gj_huffscan.cu) for frames without restart markers -- what libjpeg, PIL and OpenCV write unless asked --:
+ *   there every scan is one segment, and one thread per segment decodes it in seconds at 8K (DESIGN section 6).  Streams with
+ *   restart markers keep the choice above whatever their interval: whether the kernel pays for few long segments has not
+ *   been measured.  Clean streams of 512 MB and more (bit positions past 32 bits) stay off it.  Both kernels read K0's clean
+ *   stream: the segment-info tables serve only a frame that takes one thread per segment anyway, or a cropped one.
+ * - One thread per segment (k_huff_decode, gj_huffman.cu) otherwise; of a cropped frame only the segments that hold its
+ *   blocks, unless the sub-sequence kernel decodes the whole frame.
+ * A forced lane count (any entry) asks for the self-synchronising kernel; 1 lane per segment means one thread per segment. */
+int gj_k3_choose(const struct gj_geometry* g, int request, const int force_lanes[GJ_MAX_COMP], int positions, int crop,
+                 struct gj_huff_dec_args* a)
+{
+    const int segblk = g->seg_mcu * g->lay.bpm;
+    const int many_segments = g->seg_count >= 30000;
+    int forced = 0, forced_scan = 0;   /* a lane count is given: for any entry, for a scan of the frame */
+    a->ecs_bytes = 0;
+    for ( int k = 0; k < GJ_MAX_COMP; k++ ) {
+        forced |= force_lanes[k];
+        forced_scan |= k < g->scan_count ? force_lanes[k] : 0;
+        a->ecs_bytes += a->scan_bytes[k];
+    }
+    const size_t bytes_per_block_x10 = a->ecs_bytes * 10 / (g->coef_count / 64);
+    /* one thread per segment suits the frame better, or was asked for */
+    const int per_segment = request == GJ_K3_THREAD_PER_SEGMENT || g->lay.interleaved || segblk > GJ_K3_SYNC_MAXBLK ||
+                            (many_segments && (bytes_per_block_x10 < 80 || bytes_per_block_x10 > 200));
+    /* a lane count forced for a scan of the frame outweighs that, but not dec_opt_huffman=thread_per_segment */
+    int sync = !(forced_scan ? request == GJ_K3_THREAD_PER_SEGMENT : per_segment) && segblk <= GJ_K3_SYNC_MAXBLK;
+    for ( int k = 0; k < g->scan_count; k++ ) {
+        const int n = force_lanes[k] ? force_lanes[k]
+                      : g->seg_count <= 8000 ? 16
+                      : !many_segments ? (bytes_per_block_x10 > 100 ? 16 : 8)
+                      : 32;
+        a->scan_lanes[k] = (uint8_t)n;
+        sync &= n >= 2 && n <= 32 && !(n & (n - 1));
+        const uint32_t segs = (uint32_t)(g->lay.scan_seg_begin[k + 1] - g->lay.scan_seg_begin[k]);
+        a->scan_dense[k] = a->scan_bytes[k] / segs >= (uint32_t)(16 * segblk);
+    }
+    if ( positions == GJ_K3_SEGMENT_INFO ) {
+        if ( g->restart_interval <= 0 || (forced && !crop) || request == GJ_K3_SUBSEQUENCE || !(crop || per_segment) ) return -1;
+        a->kernel = GJ_K3_THREAD_PER_SEGMENT;
+        return crop;
+    }
+    const int subsequence = request != GJ_K3_THREAD_PER_SEGMENT && a->ecs_bytes < ((size_t)1 << 29) &&
+                            (request == GJ_K3_SUBSEQUENCE || (!forced && g->restart_interval <= 0));
+    const int pick = crop && !subsequence;
+    /* (the sub-sequence kernel takes positions from the marker list only: a resynchronised frame takes the others) */
+    a->kernel = subsequence && positions != GJ_K3_RESYNC_TABLE ? GJ_K3_SUBSEQUENCE
+                : !pick && sync                                ? GJ_K3_SELF_SYNC
+                                                               : GJ_K3_THREAD_PER_SEGMENT;
+    return pick;
+}
+
 /* ------------------------------------------------------------------------------------------- */
 /* writer                                                                                        */
 

@@ -53,8 +53,7 @@ struct gpujpeg_decoder {
     int idct_flavour;
     int flipped;                  /* dec_opt_flipped */
     unsigned channel_remap;       /* dec_opt_channel_remap: (count << 24) | selector nibbles, 0 = none */
-    int thread_per_segment;       /* dec_opt_huffman=thread_per_segment */
-    int subsequence_req;          /* dec_opt_huffman=subsequence */
+    int huffman_req;              /* dec_opt_huffman: GJ_K3_AUTO, GJ_K3_THREAD_PER_SEGMENT or GJ_K3_SUBSEQUENCE */
     int used_subsequences;        /* the last frame's Huffman stage ran the sub-sequence kernel */
     void* d_ss_scratch; size_t d_ss_scratch_size;   /* its per-segment and per-sub-sequence state */
     int force_lanes[GJ_MAX_COMP]; /* dec_opt_huffman_lanes: lanes per restart segment by scan, 0 = chosen from the frame's segment count */
@@ -668,40 +667,10 @@ static int resync_segments(struct gpujpeg_decoder* d, const struct gj_stream* st
     return rc;
 }
 
-/* Which Huffman decoder kernel (both timed by frame size and content with profiles/k3_matrix.py on an H100 SXM): a frame
- * with few segments cannot occupy the GPU with one thread per segment -- there the self-synchronising walks buy
- * parallelism INSIDE a segment (4K photo: 66 us against 102); with 30 000 segments and more the segments alone keep the
- * machine busy and the redundant walks pay off only for dense segments, 8 to 20 bytes per block (8K q90: 330 us with 32
- * lanes against 401), not at photographic q75 densities (8K: 205 against 212 with the best lane count), for very sparse
- * or for random content.  Interleaved scans: a walk that starts inside the
- * stream also has to guess which component's block it is in, and a wrong guess does not heal by itself (other Huffman
- * tables) -- exactness then spreads one lane per round; one thread per segment is faster at every size. */
-static int wants_thread_per_segment(const struct gpujpeg_decoder* d, const struct gj_geometry* g, size_t ecs_bytes)
-{
-    const size_t bytes_per_block_x10 = ecs_bytes * 10 / (g->coef_count / 64);
-    const int many_segments = g->seg_count >= 30000;
-    return d->thread_per_segment || g->lay.interleaved || g->seg_mcu * g->lay.bpm > 40 ||
-           (many_segments && (bytes_per_block_x10 < 80 || bytes_per_block_x10 > 200));
-}
-
-/* The sub-sequence kernel (gj_huffscan.cu) for frames without restart markers -- what libjpeg, PIL and OpenCV write unless
- * asked --: there every scan is one segment, and one thread per segment decodes it in seconds at 8K (DESIGN section 6).
- * Streams with restart markers keep the choice above whatever their interval: whether the new kernel pays for few long
- * segments has not been measured, and dec_opt_huffman=subsequence forces it.  Clean streams of 512 MB and more (bit positions
- * past 32 bits) stay on the thread-per-segment kernel. */
-static int wants_subsequences(const struct gpujpeg_decoder* d, const struct gj_geometry* g, size_t ecs_bytes)
-{
-    if ( d->thread_per_segment || ecs_bytes >= ((size_t)1 << 29) ) return 0;
-    if ( d->subsequence_req ) return 1;
-    for ( int k = 0; k < GJ_MAX_COMP; k++ )
-        if ( d->force_lanes[k] ) return 0;
-    return g->restart_interval <= 0;
-}
-
 /* Segment info [ref: src/gpujpeg_reader.c:1168-1215]: a stream can carry, in front of every scan, the position of every
  * restart segment.  The reference's reader then splits the scan by that table instead of searching for markers; here the
  * search is K0's job on the device, and the table only pays when K3 runs one thread per segment on the file bytes (the
- * self-synchronising kernel reads K0's clean stream): then K0 and the round trip for its report are skipped altogether.
+ * other kernels read K0's clean stream; gj_k3_choose): then K0 and the round trip for its report are skipped altogether.
  * The table is advisory: count, order and range are checked, and anything odd sends the frame down the K0 path.
  * Walks the remaining scans on the host (extents from the tables, marker segments between scans by length), fills
  * d->h_seg_off.  Returns 1 if the frame can be decoded from the tables (st / pos / adobe advanced to the end of the
@@ -711,9 +680,6 @@ static int split_by_segment_info(struct gpujpeg_decoder* d, const uint8_t* image
 {
     const struct gj_geometry* g = &d->geo;
     if ( !st->seginfo[0].pieces || g->seg_mcu <= 0 || st->restart_interval <= 0 || d->ignore_segment_info ) return 0;
-    for ( int k = 0; k < GJ_MAX_COMP && !d->crop; k++ )
-        if ( d->force_lanes[k] ) return 0;   /* the self-synchronising kernel was asked for */
-    if ( d->subsequence_req && !d->thread_per_segment ) return 0;   /* so was the sub-sequence kernel: it reads K0's clean stream */
     if ( (size_t)g->seg_count * 4 > d->seg_off_size ) {
         gj_cuda_free(d->d_seg_off);
         if ( d->h_seg_off ) gj_cuda_free_host(d->h_seg_off);
@@ -728,7 +694,7 @@ static int split_by_segment_info(struct gpujpeg_decoder* d, const uint8_t* image
     struct gj_stream t = *st;
     size_t p = *pos;
     int ad = *adobe;
-    size_t ecs_bytes = 0;
+    struct gj_huff_dec_args k3 = {0};   /* (only the scans' bytes and the choice) */
     for ( int k = 0;; k++ ) {
         if ( k >= g->scan_count || k >= t.scan_count ) return 0;
         const struct gj_seginfo* si = &t.seginfo[k];
@@ -765,7 +731,7 @@ static int split_by_segment_info(struct gpujpeg_decoder* d, const uint8_t* image
         }
         t.scan[k].end = begin + prev;
         if ( image[t.scan[k].end] != 0xFF ) return 0;   /* a marker follows the scan */
-        ecs_bytes += prev;
+        k3.scan_bytes[k] = prev;
         p = t.scan[k].end;
         const int r = gj_reader_walk(image, image_size, &p, &t, &ad);
         if ( r < 0 ) return 0;
@@ -774,7 +740,7 @@ static int split_by_segment_info(struct gpujpeg_decoder* d, const uint8_t* image
             break;
         }
     }
-    if ( !d->crop && !wants_thread_per_segment(d, g, ecs_bytes) ) return 0;   /* (a cropped frame always takes that kernel) */
+    if ( gj_k3_choose(g, d->huffman_req, d->force_lanes, GJ_K3_SEGMENT_INFO, d->crop, &k3) < 0 ) return 0;
     *st = t;
     *pos = p;
     *adobe = ad;
@@ -1536,52 +1502,34 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     ha.d_unit_ctr = d->d_k3_ctr;
     ha.d_clean = (const uint32_t*)d->d_clean;
     ha.d_list_cpos = d->d_list_cpos;
-    ha.force_thread_per_segment = d->thread_per_segment;
-    /* which kernel (wants_thread_per_segment), and for the self-synchronising one how many lanes share a restart segment
-     * (profiles/k3_matrix.py) */
-    size_t ecs_bytes = 0;
-    for ( int k = 0; k < g->scan_count; k++ )
-        ecs_bytes += st.scan[k].end - st.scan[k].begin;
-    const size_t bytes_per_block_x10 = ecs_bytes * 10 / (g->coef_count / 64);
-    const int many_segments = g->seg_count >= 30000;
-    ha.force_thread_per_segment = by_table || wants_thread_per_segment(d, g, ecs_bytes);
     for ( int k = 0; k < g->scan_count; k++ ) {
         ha.first_rank[k] = first_rank[k];
         ha.scan_cbegin[k] = scan_cbegin[k];
-        const int segs = g->lay.scan_seg_begin[k + 1] - g->lay.scan_seg_begin[k];
-        const size_t avg = (st.scan[k].end - st.scan[k].begin) / (size_t)segs;
-        ha.scan_lanes[k] = (uint8_t)(g->seg_count <= 8000 ? 16
-                                     : !many_segments     ? (bytes_per_block_x10 > 100 ? 16 : 8)
-                                     : 32);
-        if ( d->force_lanes[k] ) {   /* (never with by_table: split_by_segment_info declines then) */
-            ha.scan_lanes[k] = (uint8_t)d->force_lanes[k];
-            ha.force_thread_per_segment = d->thread_per_segment;
-        }
         ha.scan_bytes[k] = (uint32_t)(st.scan[k].end - st.scan[k].begin);
-        ha.scan_dense[k] = avg >= (size_t)16 * (size_t)(g->seg_mcu * g->lay.bpm);
     }
+    const int pick = gj_k3_choose(g, d->huffman_req, d->force_lanes,
+                                  by_table ? GJ_K3_SEGMENT_INFO : resync ? GJ_K3_RESYNC_TABLE : GJ_K3_MARKER_LIST, d->crop, &ha);
+    if ( pick < 0 ) return GPUJPEG_ERROR;   /* (not for a frame split_by_segment_info accepted: the same question) */
     ha.seg_count = g->seg_count;
     ha.lay = g->lay;
     ha.seg_mcu = g->seg_mcu;
     ha.d_coef = d->d_coef;
     ha.d_cext = d->d_cext;
     ha.d_tables = d->d_tab;
-    if ( !by_table && wants_subsequences(d, g, ecs_bytes) ) {
+    if ( ha.kernel == GJ_K3_SUBSEQUENCE ) {
         const int ctas = gj_subseq_grid();
-        const size_t need = ctas > 0 ? gj_subseq_scratch_bytes(g->seg_count, ecs_bytes, ctas) : 0;
+        const size_t need = ctas > 0 ? gj_subseq_scratch_bytes(g->seg_count, ha.ecs_bytes, ctas) : 0;
         if ( ctas <= 0 || grow_dev(&d->d_ss_scratch, &d->d_ss_scratch_size, need) ) {
             GJ_ERR("Decoder allocation failed: %s\n", gj_cuda_last_error());
             return GPUJPEG_ERROR;
         }
-        ha.subsequence = 1;
         ha.d_ss_scratch = d->d_ss_scratch;
         ha.ss_scratch_bytes = d->d_ss_scratch_size;
-        ha.ecs_bytes = ecs_bytes;
     }
-    /* a cropped frame: the blocks K4 transforms; K3 decodes the segments that hold them (gj_crop_pick), one thread per segment,
-     * unless the sub-sequence kernel decodes the whole frame */
+    /* a cropped frame: the blocks K4 transforms; K3 decodes the segments that hold them (gj_crop_pick), unless the
+     * sub-sequence kernel decodes the whole frame */
     if ( d->crop ) crop_blocks(d);
-    if ( d->crop && !ha.subsequence ) {
+    if ( pick ) {
         if ( grow_pick(d, (size_t)g->seg_count) ) {
             GJ_ERR("Decoder allocation failed: %s\n", gj_cuda_last_error());
             return GPUJPEG_ERROR;
@@ -1601,7 +1549,9 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     d->last_progressive = 0;
   for ( int pass = 0;; pass++ ) {
     if ( resync ) {
-        if ( resync_segments(d, &st, first_rank, end_rank, scan_cbegin, &ha) ) return GPUJPEG_ERROR;
+        if ( resync_segments(d, &st, first_rank, end_rank, scan_cbegin, &ha) ||
+             gj_k3_choose(g, d->huffman_req, d->force_lanes, GJ_K3_RESYNC_TABLE, d->crop, &ha) < 0 )   /* (the same pick) */
+            return GPUJPEG_ERROR;
         d->last_args = ha;
     }
     /* host output of a large frame leaves stripe by stripe (decode_striped): K4 per stripe and, where the Huffman decoder can
@@ -1612,7 +1562,9 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
         const char* v = getenv("GPUJPEG_B200_STRIPES_K3");
         d->k3_parts = !(v && v[0] == '0');
     }
-    const int k3_striped = striped && d->k3_parts && !resync && gj_huffman_decode_parts_eligible(&ha);
+    /* (part_seg_lo / part_seg_hi: the self-synchronising kernel on 4:4:4 frames with one scan per component, positions from
+     * the marker list) */
+    const int k3_striped = striped && d->k3_parts && ha.kernel == GJ_K3_SELF_SYNC && !resync && g->lay.simple && !g->lay.interleaved;
     /* a cropped frame leaves blocks undecoded: their extent 0 makes them read as zero (the rule of gj_internal.h) */
     if ( d->crop && gj_cuda_memset_async(d->d_cext, 0, g->coef_count / 64, d->stream) ) {
         GJ_ERR("Decoder extent clear failed: %s\n", gj_cuda_last_error());
@@ -1648,7 +1600,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     }
     break;
   }
-    d->used_subsequences = ha.subsequence && !ha.d_seg_tab;
+    d->used_subsequences = ha.kernel == GJ_K3_SUBSEQUENCE;
     output->metadata = &d->metadata;
 
     record_stats(d, output, &pi, stats, t_reader_ms, t_begin);
@@ -1785,15 +1737,9 @@ int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt,
         return GPUJPEG_NOERR;
     }
     if ( strcmp(opt, GPUJPEG_DEC_OPT_HUFFMAN) == 0 ) {
-        if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_AUTO) == 0 ) decoder->thread_per_segment = decoder->subsequence_req = 0;
-        else if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_THREAD_PER_SEGMENT) == 0 ) {
-            decoder->thread_per_segment = 1;
-            decoder->subsequence_req = 0;
-        }
-        else if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_SUBSEQUENCE) == 0 ) {
-            decoder->thread_per_segment = 0;
-            decoder->subsequence_req = 1;
-        }
+        if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_AUTO) == 0 ) decoder->huffman_req = GJ_K3_AUTO;
+        else if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_THREAD_PER_SEGMENT) == 0 ) decoder->huffman_req = GJ_K3_THREAD_PER_SEGMENT;
+        else if ( strcmp(val, GPUJPEG_DEC_HUFFMAN_VAL_SUBSEQUENCE) == 0 ) decoder->huffman_req = GJ_K3_SUBSEQUENCE;
         else {
             GJ_ERR("Unknown Huffman decoder kernel: %s\n", val);
             return GPUJPEG_ERROR;

@@ -51,7 +51,7 @@ namespace {
 constexpr unsigned FULL = 0xFFFFFFFFu;
 constexpr int SD_WARPS = 16;
 constexpr int SD_THREADS = SD_WARPS * 32;
-constexpr int SD_MAXBLK = 40;          // blocks per restart segment this kernel takes (every RESTART_AUTO setting)
+constexpr int SD_MAXBLK = GJ_K3_SYNC_MAXBLK;   // blocks per restart segment this kernel takes
 constexpr int SD_MAXLEN = 32760;       // clean bytes of a segment that are looked at (a valid 40-block segment has < 18 KB)
 constexpr int SD_MINSUB = 8;           // shortest sub-sequence, bytes
 constexpr int SD_HEAD = 16;            // M_SPLIT: coefficients of a block (zig-zag order) that are staged in shared memory
@@ -861,20 +861,14 @@ k_huff_decode_sync(const __grid_constant__ SdParams P)
 
 }  // namespace
 
-/* Can the self-synchronising kernel take this frame?  (segments of at most SD_MAXBLK blocks, K0's clean stream and
- * the per-scan lane counts present) */
-extern "C" int gj_huffman_decode_sync_eligible(const struct gj_huff_dec_args* a)
-{
-    if ( !a->d_clean || !a->d_list_cpos || !a->d_unit_ctr || a->seg_mcu * a->lay.bpm > SD_MAXBLK ) return 0;
-    for ( int s = 0; s < a->lay.scan_count; s++ ) {
-        const int n = a->scan_lanes[s];
-        if ( n < 2 || n > 32 || (n & (n - 1)) ) return 0;   // (one lane per segment: k_huff_decode)
-    }
-    return 1;
-}
-
 extern "C" int gj_launch_huffman_decode_sync(const struct gj_huff_dec_args* a, gj_stream_t stream)
 {
+    /* segments of at most SD_MAXBLK blocks, K0's clean stream and a valid lane count for every scan */
+    if ( !a->d_clean || !a->d_list_cpos || !a->d_unit_ctr || a->seg_mcu * a->lay.bpm > SD_MAXBLK ) return -1;
+    for ( int s = 0; s < a->lay.scan_count; s++ ) {
+        const int n = a->scan_lanes[s];
+        if ( n < 2 || n > 32 || (n & (n - 1)) ) return -1;
+    }
     SdParams P;
     P.lay = a->lay;
     P.clean = a->d_clean;

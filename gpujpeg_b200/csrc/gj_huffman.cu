@@ -1374,31 +1374,23 @@ extern "C" int gj_launch_huffman_stats(const struct gj_huff_enc_args* a, uint64_
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
-extern "C" int gj_huffman_decode_sync_eligible(const struct gj_huff_dec_args* a);
 extern "C" int gj_launch_huffman_decode_sync(const struct gj_huff_dec_args* a, gj_stream_t stream);
-
-/* can the frame be decoded in several launches (part_seg_lo / part_seg_hi of the arguments)?  The self-synchronising kernel on
- * 4:4:4 frames with one scan per component, positions from the marker list */
-extern "C" int gj_huffman_decode_parts_eligible(const struct gj_huff_dec_args* a)
-{
-    return !a->force_thread_per_segment && !a->subsequence && gj_huffman_decode_sync_eligible(a) && !a->d_seg_tab && a->lay.simple &&
-           !a->lay.interleaved;
-}
 
 extern "C" int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_stream_t stream)
 {
-    /* segments of any length, several threads per segment (gj_huffscan.cu): whole segments, a cropped frame included; the
-     * number of every restart marker is checked first, as a full decode by the kernels below would */
-    if ( a->subsequence && !a->d_seg_off && !a->d_seg_tab ) {
+    switch ( a->kernel ) {
+    case GJ_K3_SUBSEQUENCE:
+        /* segments of any length, several threads per segment (gj_huffscan.cu): whole segments, a cropped frame included;
+         * the number of every restart marker is checked first, as a full decode by the other kernels would */
         if ( a->seg_count > a->lay.scan_count &&
              gj_launch_pdl(k_rst_check, dim3((a->seg_count + 255) / 256), dim3(256), 0, stream, *a) != cudaSuccess )
             return -1;
         return gj_launch_huffman_decode_subseq(a, a->d_ss_scratch, a->ss_scratch_bytes, a->ecs_bytes, stream);
+    case GJ_K3_SELF_SYNC: return gj_launch_huffman_decode_sync(a, stream);   /* several lanes per segment (gj_huffdec.cu) */
+    case GJ_K3_THREAD_PER_SEGMENT: break;                                      /* one thread per segment: below */
+    default: return -1;
     }
     const bool pick = a->d_pick != nullptr;
-    /* restart segments of at most 40 blocks (every RESTART_AUTO setting): several lanes per segment, self-synchronising
-     * (gj_huffdec.cu); longer segments: one thread per segment (below).  A cropped frame always takes the latter. */
-    if ( !pick && !a->force_thread_per_segment && gj_huffman_decode_sync_eligible(a) ) return gj_launch_huffman_decode_sync(a, stream);
     if ( pick && !a->d_seg_off && !a->d_seg_tab ) {
         if ( gj_launch_pdl(k_rst_check, dim3((a->seg_count + 255) / 256), dim3(256), 0, stream, *a) != cudaSuccess ) return -1;
         if ( a->pick_count == 0 ) return 0;

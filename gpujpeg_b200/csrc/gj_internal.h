@@ -458,12 +458,11 @@ struct gj_huff_dec_args {
     const uint32_t* d_clean;
     const uint32_t* d_list_cpos;
     uint32_t scan_cbegin[GJ_MAX_COMP];
-    /* self-synchronising decoder: lanes that share one restart segment in scan s (4, 8, 16 or 32), from the scan's
-     * average segment size; 0 = not computed (the thread-per-segment kernel is used) */
+    /* self-synchronising kernel: lanes that share one restart segment in scan s (2, 4, 8, 16 or 32; gj_k3_choose) */
     uint8_t scan_lanes[GJ_MAX_COMP];
     uint32_t scan_bytes[GJ_MAX_COMP];  /* entropy-coded bytes of scan s (as in the file) */
     uint8_t scan_dense[GJ_MAX_COMP];   /* >= 16 bytes of entropy-coded data per block: worth staging blocks in shared memory */
-    int force_thread_per_segment;   /* dec_opt_huffman=thread_per_segment: always the one-thread-per-segment kernel */
+    int kernel;                 /* GJ_K3_THREAD_PER_SEGMENT, GJ_K3_SELF_SYNC or GJ_K3_SUBSEQUENCE (gj_k3_choose) */
     /* the decoder's stripe pipeline (self-synchronising kernel only): this launch decodes scan s's segments
      * [part_seg_lo[s], part_seg_hi[s]) -- rounded outwards to whole units, so launches must hand over at multiples of 32
      * segments --, part_seg_hi[s] == 0: all of the scan */
@@ -485,11 +484,22 @@ struct gj_huff_dec_args {
     /* the sub-sequence kernel (gj_huffscan.cu) for every scan: segments of any length, several threads per segment; positions
      * from the marker list only.  d_ss_scratch holds gj_subseq_scratch_bytes(seg_count, ecs_bytes, gj_subseq_grid()) bytes.
      * A cropped frame decodes whole segments then (d_pick is not used). */
-    int subsequence;
     void* d_ss_scratch;
     size_t ss_scratch_bytes, ecs_bytes;
 };
 int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_stream_t stream);
+/* K3's kernel.  GJ_K3_AUTO is a request only (dec_opt_huffman=auto). */
+enum { GJ_K3_AUTO = 0, GJ_K3_THREAD_PER_SEGMENT = 1, GJ_K3_SELF_SYNC = 2, GJ_K3_SUBSEQUENCE = 3 };
+/* where K3 finds the restart segments: K0's marker list, the stream's segment-info tables, the resynchronised table */
+enum { GJ_K3_MARKER_LIST = 0, GJ_K3_SEGMENT_INFO = 1, GJ_K3_RESYNC_TABLE = 2 };
+#define GJ_K3_SYNC_MAXBLK 40   /* blocks per restart segment the self-synchronising kernel takes (every RESTART_AUTO setting) */
+/* The one place K3's kernel is chosen (gj_codestream.c), from the frame (geometry, a->scan_bytes), the request
+ * (dec_opt_huffman: GJ_K3_AUTO, GJ_K3_THREAD_PER_SEGMENT or GJ_K3_SUBSEQUENCE; dec_opt_huffman_lanes: force_lanes, 0 =
+ * automatic), where the segment positions come from (GJ_K3_MARKER_LIST ..) and whether the frame is cropped.  Sets
+ * a->kernel, scan_lanes and scan_dense of the frame's scans, ecs_bytes.  Returns 1 if K3 decodes only the segments of a crop
+ * (gj_crop_pick), 0 if every segment, -1 for GJ_K3_SEGMENT_INFO if the frame is not to be decoded from those tables. */
+int gj_k3_choose(const struct gj_geometry* g, int request, const int force_lanes[GJ_MAX_COMP], int positions, int crop,
+                 struct gj_huff_dec_args* a);
 /* sub-sequence kernel: bytes per sub-sequence (a tuning value; GPUJPEG_B200_SUBSEQ_BYTES overrides it for experiments), the
  * smallest value the scratch is sized for, warm-up of a sub-sequence's first walk */
 #define GJ_SS_SUB_BYTES 32
@@ -500,7 +510,6 @@ int gj_subseq_grid(void);   /* CTAs of its cooperative grid on the current devic
 int gj_subseq_rounds(const void* d_scratch, gj_stream_t stream);   /* rounds of the last launch on that scratch */
 int gj_launch_huffman_decode_subseq(const struct gj_huff_dec_args* a, void* d_scratch, size_t scratch_bytes, size_t ecs_bytes,
                                     gj_stream_t stream);
-int gj_huffman_decode_parts_eligible(const struct gj_huff_dec_args* a);   /* part_seg_lo / part_seg_hi may be used */
 
 /* Progressive frames (gj_progressive.cu): one scan of a SOF2 frame as k_prog_decode sees it.  An interleaved scan (DC
  * only) codes MCUs of the frame's MCU grid; a non-interleaved one codes the component's own ceil(w_c/8) x ceil(h_c/8)

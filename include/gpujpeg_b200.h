@@ -482,7 +482,8 @@ GPUJPEG_API int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size
  * sub-sequences of 32 bytes, one per thread, synchronised over the whole scan; otherwise several lanes per restart segment,
  * self-synchronising, for segments of at most 40 blocks, one thread per segment for longer ones.  "thread_per_segment":
  * always the latter two.  "subsequence": the sub-sequence kernel for every baseline scan.  Streams decoded from their
- * segment-info tables and resynchronised streams take the thread-per-segment kernel; progressive scans their own.
+ * segment-info tables take the thread-per-segment kernel; a resynchronised stream (broken restart-marker numbering) the
+ * self-synchronising or the thread-per-segment kernel, chosen as for a stream with restart markers; progressive scans their own.
  * On damaged entropy-coded data the kernels can differ: the sub-sequence kernel reads the bits past a restart segment's end
  * as zeros (as libjpeg does), the thread-per-segment kernel reads the bytes that follow the segment.  A code no Huffman table
  * holds consumes 16 bits and reads as symbol 0 in every kernel. */
@@ -490,8 +491,10 @@ GPUJPEG_API int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size
 #define GPUJPEG_DEC_HUFFMAN_VAL_AUTO "auto"
 #define GPUJPEG_DEC_HUFFMAN_VAL_THREAD_PER_SEGMENT "thread_per_segment"
 #define GPUJPEG_DEC_HUFFMAN_VAL_SUBSEQUENCE "subsequence"
-/* extension (tuning): lanes that share one restart segment in the self-synchronising decoder: 0 = chosen per scan from
- * the scan's bytes per segment (default), or 4, 8, 16, 32 for every scan */
+/* extension (tuning): lanes that share one restart segment in the self-synchronising decoder: 0 = chosen from the frame's
+ * segment count and bytes per block (default), or 2, 4, 8, 16, 32 -- one number for every scan or a comma-separated list
+ * by scan.  A forced count asks for the self-synchronising kernel wherever it can take the frame (segments of at most 40
+ * blocks, no crop) and dec_opt_huffman asks for no other; 1 lane per segment is the thread-per-segment kernel. */
 #define GPUJPEG_DEC_OPT_HUFFMAN_LANES "dec_opt_huffman_lanes"
 /* Extension of this build (not in the reference): scaled decoding.  "1" (default), "1/2", "1/4" or "1/8": the decoder
  * returns an image of ceil(W / s) x ceil(H / s) pixels (in output->param_image and data_size, for every output type),
