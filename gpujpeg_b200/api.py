@@ -194,8 +194,10 @@ def _ptr(x):
 class Encoder:
     """gpujpeg_encoder_create / gpujpeg_encoder_encode / gpujpeg_encoder_destroy"""
 
-    def __init__(self, stream=0, pinned_output=False, huffman="standard"):
-        """huffman: "standard" (the Annex K tables) or "optimized" (tables fitted to every frame, enc_opt_huffman)"""
+    def __init__(self, stream=0, pinned_output=False, huffman="standard", writer="gpujpeg"):
+        """huffman: "standard" (the Annex K tables) or "optimized" (tables fitted to every frame, enc_opt_huffman).
+        writer: "gpujpeg" (this library's stream) or "libjpeg" (the file libjpeg-turbo -- PIL, torchvision, OpenCV -- writes with
+        its defaults, byte for byte; enc_opt_writer)"""
         self._h = lib.gpujpeg_encoder_create(C.c_void_p(stream))
         if not self._h:
             raise GpuJpegError("gpujpeg_encoder_create failed (no CUDA device?)")
@@ -203,10 +205,15 @@ class Encoder:
             self.set_option("enc_opt_out", "enc_out_val_pinned")
         if huffman != "standard":
             self.set_option("enc_opt_huffman", huffman)
+        self.writer = "gpujpeg"
+        if writer != "gpujpeg":
+            self.set_option("enc_opt_writer", writer)
 
     def set_option(self, key, val):
         if lib.gpujpeg_encoder_set_option(self._h, key.encode(), val.encode()) != 0:
             raise GpuJpegError("gpujpeg_encoder_set_option(%s, %s) failed" % (key, val))
+        if key == "enc_opt_writer":
+            self.writer = val
 
     def encode_raw(self, image, param, param_image, device=None):
         """returns (address, size) of the encoder-owned JPEG buffer (valid until the next call)"""
@@ -221,9 +228,14 @@ class Encoder:
             raise GpuJpegError("gpujpeg_encoder_encode failed (%d)" % rc)
         return out.value, size.value
 
-    def encode(self, image, quality=75, restart_interval=RESTART_AUTO, interleaved=0, width=None, height=None,
+    def _interleaved(self, interleaved):
+        """None: the writer's default -- 0 (one scan per component) for gpujpeg, 1 (libjpeg's single scan) for libjpeg"""
+        return (1 if self.writer == "libjpeg" else 0) if interleaved is None else interleaved
+
+    def encode(self, image, quality=75, restart_interval=RESTART_AUTO, interleaved=None, width=None, height=None,
                width_padding=0, verbose=0, subsampling="4:4:4", segment_info=0):
         """image: HxWx3 uint8 numpy array / torch tensor (host or cuda).  Returns the JPEG as numpy uint8 (a copy)."""
+        interleaved = self._interleaved(interleaved)
         if width is None:
             height, width = image.shape[0], image.shape[1]
         p = default_parameters(quality, restart_interval, interleaved, subsampling)
@@ -232,13 +244,13 @@ class Encoder:
         addr, size = self.encode_raw(image, p, image_parameters(width, height, width_padding))
         return np.ctypeslib.as_array((C.c_uint8 * size).from_address(addr)).copy()
 
-    def encode_samples(self, raw, width, height, pixel_format, quality=75, restart_interval=RESTART_AUTO, interleaved=0,
+    def encode_samples(self, raw, width, height, pixel_format, quality=75, restart_interval=RESTART_AUTO, interleaved=None,
                        color_space=GPUJPEG_YCBCR_JPEG, subsampling=None, alpha=False, color_space_internal=None):
         """raw: flat uint8 buffer in `pixel_format` / `color_space`.  With the JPEG colour space and subsampling=None the
         samples go into the JPEG as they are (the JPEG takes the format's sampling); other colour spaces are
         transformed, and `subsampling` ("4:2:0", ...) selects a JPEG sampling other than the format's.  Returns the
         JPEG bytes."""
-        p = default_parameters(quality, restart_interval, interleaved, subsampling or "4:4:4")
+        p = default_parameters(quality, restart_interval, self._interleaved(interleaved), subsampling or "4:4:4")
         if subsampling == "4:4:4":
             lib.gpujpeg_parameters_chroma_subsampling(C.byref(p), 0x11111100)
         if alpha:   # comp_count = 4: the alpha samples of a 4444-u8-p0123 image become a fourth component (first one's sampling)

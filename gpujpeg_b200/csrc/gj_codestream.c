@@ -536,6 +536,8 @@ static int comp_id(const struct gpujpeg_parameters* param, int c)
 /* Everything before the first SOS.  The header flavour follows the internal colour space unless the caller forces one
  * (enc_hdr option): SPIFF names the colour space (BT.601 / BT.709 need it), Adobe APP14 marks RGB, JFIF is the default for
  * YCbCr JPEG, Exif on request (gj_exif.c).  An orientation goes into the SPIFF directory or the Exif header.
+ * extras->libjpeg (enc_opt_writer=libjpeg, a JFIF frame): the segments libjpeg's jcmarker.c writes after jpeg_set_defaults --
+ * JFIF 1.01 with a 1:1 aspect ratio, DRI only for a non-zero interval, no COM.
  * [ref: src/gpujpeg_writer.c:451-518] */
 size_t gj_write_header(uint8_t* out, const struct gpujpeg_parameters* param,
                        const struct gpujpeg_image_parameters* pi, const uint8_t raw_q[2][64],
@@ -543,6 +545,7 @@ size_t gj_write_header(uint8_t* out, const struct gpujpeg_parameters* param,
                        const struct gj_header_extras* extras)
 {
     uint8_t* p = out;
+    const int libjpeg = extras && extras->libjpeg;
     p = wmark(p, 0xD8);
     const int oriented = extras && extras->metadata.vals[GPUJPEG_METADATA_ORIENTATION].set;
     if ( header_type == GPUJPEG_HEADER_DEFAULT )   /* four components and an orientation need SPIFF to be described */
@@ -609,9 +612,16 @@ size_t gj_write_header(uint8_t* out, const struct gpujpeg_parameters* param,
         p += 5;
         p = w8(p, 1);
         p = w8(p, 1);
-        p = w8(p, 1);
-        p = w16(p, 300);
-        p = w16(p, 300);
+        if ( libjpeg ) {   /* jpeg_set_defaults: density unit 0, aspect ratio 1:1 */
+            p = w8(p, 0);
+            p = w16(p, 1);
+            p = w16(p, 1);
+        }
+        else {
+            p = w8(p, 1);
+            p = w16(p, 300);
+            p = w16(p, 300);
+        }
         p = w8(p, 0);
         p = w8(p, 0);
     }
@@ -654,6 +664,14 @@ size_t gj_write_header(uint8_t* out, const struct gpujpeg_parameters* param,
             memcpy(p, s->vals, s->nvals);
             p += s->nvals;
         }
+    }
+    if ( libjpeg ) {   /* jcmarker.c: a DRI segment only for a non-zero interval, no comment */
+        if ( param->restart_interval > 0 ) {
+            p = wmark(p, 0xDD);
+            p = w16(p, 4);
+            p = w16(p, param->restart_interval);
+        }
+        return (size_t)(p - out);
     }
     p = wmark(p, 0xDD);
     p = w16(p, 4);

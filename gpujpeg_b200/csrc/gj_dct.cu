@@ -478,6 +478,234 @@ k_fdct_rgb_ss(const uint8_t* __restrict__ raw, int width, int height, size_t pit
     }
 }
 
+/* ------------------------------------------------------------------------------------------- */
+/* K1 of enc_opt_writer=libjpeg: the coefficients libjpeg-turbo quantises (gj_rgb_ycc_libjpeg, gj_down_libjpeg,
+ * gj_fdct_islow_block, gj_quant_libjpeg).  NC = 3: RGB u8 interleaved, luminance HS x VS, chrominance 1x1; NC = 1: grey u8.
+ * A CTA owns one MCU row of a 512-pixel strip, as k_fdct_rgb_ss (a strip holds whole MCUs, so the pairs a downsampler averages
+ * never cross it).  Colour phase: 4 pixels per thread, int32, luminance and FULL-resolution chrominance staged as bytes.
+ * Transform phase: one thread per block; it reads its samples with libjpeg's edge rules -- columns clamped to the last pixel of
+ * the row, full-resolution rows to the last row of the image, downsampled rows to the component's last real row -- downsamples,
+ * transforms and quantises in registers.  Blocks past a component's width_in_blocks / height_in_blocks (the dummy blocks of
+ * interleaved MCUs, jccoefct.c) carry only a DC: that of the last real block to their left, or, in a block row below the
+ * component's last, that of the MCU's rightmost block in the last real row.  Both sources lie in the same CTA. */
+struct LjGrid {
+    int bcx[3], bcy[3], blk_off[3];   /* the block grids of the MCU-row range launched (as SsGrid) */
+    int wib[3], hib[3];               /* width_in_blocks, and height_in_blocks counted from the range's first block row */
+};
+struct LjParams {
+    uint32_t recip[2][64];            /* gj_quant_recip_libjpeg of the quantiser, zig-zag order */
+    uint16_t q[2][64];
+};
+
+template <int HS, int VS, int NC>
+struct LjShape {
+    static constexpr int NTS = TB * VS + (NC == 3 ? 2 * TB / HS : 0);   // threads = blocks per CTA
+    static constexpr int CB = TB / HS;                                    // chrominance blocks per component
+    static constexpr int PLANE = 8 * VS * STRIP_PX;                       // bytes per staged plane
+    static constexpr int OUT = NTS * K1_OUT_STRIDE * 16;
+    static constexpr int SMEM = (NC * PLANE > OUT ? NC * PLANE : OUT) + NTS * 4;
+};
+
+/* n (8 or 16) bytes of a staged row from column x on, columns clamped to vw - 1 */
+template <int N>
+__device__ __forceinline__ void lj_row(const uint8_t* __restrict__ row, int x, int vw, int (&out)[N])
+{
+    if ( x + N <= vw ) {
+        const uint32_t* w = reinterpret_cast<const uint32_t*>(row + x);
+#pragma unroll
+        for ( int i = 0; i < N / 4; i++ ) {
+            const uint32_t v = w[i];
+#pragma unroll
+            for ( int j = 0; j < 4; j++ )
+                out[4 * i + j] = (int)((v >> (8 * j)) & 255u);
+        }
+    }
+    else {
+#pragma unroll
+        for ( int i = 0; i < N; i++ )
+            out[i] = row[min(x + i, vw - 1)];
+    }
+}
+
+template <int HS, int VS, int NC, int VEC>
+__global__ void __launch_bounds__(LjShape<HS, VS, NC>::NTS)
+k_fdct_libjpeg(const uint8_t* __restrict__ raw, int width, int height, size_t pitch, int16_t* __restrict__ coef,
+               uint64_t* __restrict__ nzmask, const __grid_constant__ LjGrid grid, const __grid_constant__ LjParams prm)
+{
+    gj_pdl_wait();
+    using S = LjShape<HS, VS, NC>;
+    constexpr int NTS = S::NTS, CB = S::CB;
+    constexpr int GPR = STRIP_PX / 4;                      // 4-pixel groups per row
+    constexpr int ITERS = (8 * VS * GPR + NTS - 1) / NTS;
+    extern __shared__ __align__(16) uint8_t smem[];
+    int* const s_dc = reinterpret_cast<int*>(smem + (S::SMEM - NTS * 4));
+
+    const int bx0 = blockIdx.x * TB;
+    const int x0 = bx0 * 8;
+    const int y0 = blockIdx.y * 8 * VS;
+    const int vw = min(STRIP_PX, width - x0);             // >= 1: every strip starts inside the image
+    const int vh = min(8 * VS, height - y0);              // >= 1: every MCU row starts inside the image
+    const uint8_t* src = raw + (size_t)y0 * pitch + (size_t)x0 * NC;
+
+    /* colour phase */
+#pragma unroll 4
+    for ( int it = 0; it < ITERS; it++ ) {
+        const int g = threadIdx.x + it * NTS;
+        const int row = g / GPR, gx = g % GPR, px0 = gx * 4;
+        if ( row >= 8 * VS || row >= vh || px0 >= vw ) continue;
+        const uint8_t* p = src + (size_t)row * pitch + (size_t)px0 * NC;
+        uint32_t w[NC];
+        if ( VEC == 4 && px0 + 4 <= vw ) {
+#pragma unroll
+            for ( int i = 0; i < NC; i++ )
+                w[i] = __ldg(reinterpret_cast<const uint32_t*>(p) + i);
+        }
+        else {
+            const int nb = min(4 * NC, (vw - px0) * NC);   // never read past the end of the row
+#pragma unroll
+            for ( int i = 0; i < NC; i++ )
+                w[i] = 0;
+#pragma unroll
+            for ( int i = 0; i < 4 * NC; i++ )
+                if ( i < nb ) w[i >> 2] |= (uint32_t)__ldg(p + i) << (8 * (i & 3));
+        }
+        const int off = row * STRIP_PX + px0;
+        if constexpr ( NC == 1 ) {
+            *reinterpret_cast<uint32_t*>(smem + off) = w[0];
+        }
+        else {
+            uint32_t yw = 0, cbw = 0, crw = 0;
+#pragma unroll
+            for ( int j = 0; j < 4; j++ ) {
+                const int r = (w[(3 * j) >> 2] >> (8 * ((3 * j) & 3))) & 255;
+                const int gg = (w[(3 * j + 1) >> 2] >> (8 * ((3 * j + 1) & 3))) & 255;
+                const int b = (w[(3 * j + 2) >> 2] >> (8 * ((3 * j + 2) & 3))) & 255;
+                int y, cb, cr;
+                gj_rgb_ycc_libjpeg(r, gg, b, y, cb, cr);
+                yw |= (uint32_t)y << (8 * j);
+                cbw |= (uint32_t)cb << (8 * j);
+                crw |= (uint32_t)cr << (8 * j);
+            }
+            *reinterpret_cast<uint32_t*>(smem + off) = yw;
+            *reinterpret_cast<uint32_t*>(smem + S::PLANE + off) = cbw;
+            *reinterpret_cast<uint32_t*>(smem + 2 * S::PLANE + off) = crw;
+        }
+    }
+    __syncthreads();
+
+    /* transform phase: thread t = block (comp, bx, by), lbx / lby its place in the CTA */
+    int comp, lbx, lby, bx, by;
+    if ( threadIdx.x < TB * VS ) {
+        comp = 0;
+        lbx = threadIdx.x & (TB - 1);
+        lby = threadIdx.x / TB;
+        bx = bx0 + lbx;
+        by = blockIdx.y * VS + lby;
+    }
+    else {
+        const int u = threadIdx.x - TB * VS;
+        comp = 1 + u / CB;
+        lbx = u % CB;
+        lby = 0;
+        bx = bx0 / HS + lbx;
+        by = blockIdx.y;
+    }
+    const bool active = bx < grid.bcx[comp] && by < grid.bcy[comp];
+    const bool dummy = bx >= grid.wib[comp] || by >= grid.hib[comp];
+    int v[64];
+    if ( active && !dummy ) {
+        const uint8_t* plane = smem + comp * S::PLANE;
+        if ( comp == 0 || (HS == 1 && VS == 1) ) {
+#pragma unroll
+            for ( int r = 0; r < 8; r++ ) {
+                int px[8];
+                lj_row<8>(plane + min(lby * 8 + r, vh - 1) * STRIP_PX, lbx * 8, vw, px);
+#pragma unroll
+                for ( int c = 0; c < 8; c++ )
+                    v[8 * r + c] = px[c] - 128;
+            }
+        }
+        else {
+            const int real_rows = (vh + VS - 1) / VS;   // the component's real rows in this MCU row
+#pragma unroll
+            for ( int r = 0; r < 8; r++ ) {
+                const int cy = min(r, real_rows - 1);
+                int a[8 * HS], b[8 * HS];
+                lj_row<8 * HS>(plane + min(VS * cy, vh - 1) * STRIP_PX, lbx * 8 * HS, vw, a);
+                if ( VS == 2 ) lj_row<8 * HS>(plane + min(VS * cy + 1, vh - 1) * STRIP_PX, lbx * 8 * HS, vw, b);
+#pragma unroll
+                for ( int c = 0; c < 8; c++ ) {
+                    const int i = HS * c;
+                    v[8 * r + c] = gj_down_libjpeg(HS, VS, c, a[i], a[i + HS - 1], VS == 2 ? b[i] : 0, VS == 2 ? b[i + HS - 1] : 0) - 128;
+                }
+            }
+        }
+    }
+    __syncthreads();   // the samples are in registers: the staging area becomes the output staging area
+    uint32_t packed[32];
+    uint64_t nz = 0;
+    const int tbl = comp == 0 ? 0 : 1;
+    if ( active && !dummy ) {
+        gj_fdct_islow_block(v);
+        uint32_t mlo = 0, mhi = 0;
+#pragma unroll
+        for ( int k = 0; k < 64; k += 2 ) {
+            const int q0 = gj_quant_libjpeg(v[gj_zz2nat(k)], prm.q[tbl][k], prm.recip[tbl][k]);
+            const int q1 = gj_quant_libjpeg(v[gj_zz2nat(k + 1)], prm.q[tbl][k + 1], prm.recip[tbl][k + 1]);
+            packed[k >> 1] = ((uint32_t)q0 & 0xFFFFu) | (uint32_t)q1 << 16;
+            const uint32_t bits = (q0 != 0 ? 1u : 0u) | (q1 != 0 ? 2u : 0u);
+            if ( k < 32 ) mlo |= bits << k;
+            else mhi |= bits << (k - 32);
+        }
+        nz = (uint64_t)mhi << 32 | mlo;
+        s_dc[threadIdx.x] = (int)(int16_t)(packed[0] & 0xFFFFu);
+    }
+    __syncthreads();
+    if ( active && dummy ) {
+        /* the source block: (wib - 1, by) right of the image, else the MCU's rightmost block (or the last real one) of the
+         * component's last real row */
+        const int hs_c = comp == 0 ? HS : 1, vs_c = comp == 0 ? VS : 1;
+        const int sx = by < grid.hib[comp] ? grid.wib[comp] - 1 : min(bx / hs_c * hs_c + hs_c - 1, grid.wib[comp] - 1);
+        const int sy = by < grid.hib[comp] ? lby : grid.hib[comp] - 1 - blockIdx.y * vs_c;
+        const int slot = comp == 0 ? sy * TB + (sx - bx0) : TB * VS + (comp - 1) * CB + (sx - bx0 / HS);
+        const int dc = s_dc[slot];
+        packed[0] = (uint32_t)dc & 0xFFFFu;
+#pragma unroll
+        for ( int i = 1; i < 32; i++ )
+            packed[i] = 0;
+        nz = dc != 0 ? 1u : 0u;
+    }
+    uint4* const s_out = reinterpret_cast<uint4*>(smem);
+    if ( active ) {
+        nzmask[(size_t)grid.blk_off[comp] + (size_t)by * grid.bcx[comp] + bx] = nz;
+#pragma unroll
+        for ( int i = 0; i < 8; i++ )
+            s_out[threadIdx.x * K1_OUT_STRIDE + i] = make_uint4(packed[4 * i], packed[4 * i + 1], packed[4 * i + 2], packed[4 * i + 3]);
+    }
+    __syncthreads();
+#pragma unroll
+    for ( int k = 0; k < 8; k++ ) {
+        const int q = threadIdx.x + k * NTS;
+        const int slot = q >> 3, part = q & 7;
+        int c2, bx2, by2;
+        if ( slot < TB * VS ) {
+            c2 = 0;
+            bx2 = bx0 + (slot & (TB - 1));
+            by2 = blockIdx.y * VS + slot / TB;
+        }
+        else {
+            const int u = slot - TB * VS;
+            c2 = 1 + u / CB;
+            bx2 = bx0 / HS + u % CB;
+            by2 = blockIdx.y;
+        }
+        if ( bx2 < grid.bcx[c2] && by2 < grid.bcy[c2] ) {
+            const size_t bi = (size_t)grid.blk_off[c2] + (size_t)by2 * grid.bcx[c2] + bx2;
+            reinterpret_cast<uint4*>(coef + bi * 64)[part] = s_out[slot * K1_OUT_STRIDE + part];
+        }
+    }
+}
+
 /* =========================================================================================== */
 /* K4                                                                                            */
 
@@ -1349,6 +1577,66 @@ extern "C" int gj_launch_fdct_rgb_ss(const uint8_t* d_raw, int width, int height
     const int vs = comp[0].vs > 0 ? comp[0].vs : 1;
     return gj_launch_fdct_rgb_ss_rows(d_raw, width, height, pitch, d_coef, d_nzmask, comp, 0, (comp[0].bcy + vs - 1) / vs, h_tables,
                                       stream);
+}
+
+/* ---- enc_opt_writer=libjpeg ---- */
+extern "C" int gj_launch_fdct_libjpeg_rows(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
+                                           const struct gj_comp_geo* comp, int comp_count, int my0, int my1, const uint8_t raw_q[2][64],
+                                           gj_stream_t stream)
+{
+    const int hs = comp[0].hs, vs = comp[0].vs;
+    if ( comp_count != 1 && comp_count != 3 ) return -1;
+    if ( comp_count == 3 && (comp[1].hs != 1 || comp[1].vs != 1 || comp[2].hs != 1 || comp[2].vs != 1) ) return -1;
+    if ( comp_count == 1 && (hs != 1 || vs != 1) ) return -1;
+    const int mcu_rows = (comp[0].bcy + vs - 1) / vs;
+    if ( my0 < 0 || my1 > mcu_rows || my0 >= my1 ) return -1;
+    LjGrid lg;
+    memset(&lg, 0, sizeof lg);
+    for ( int c = 0; c < comp_count; c++ ) {
+        const int per = c == 0 ? vs : 1;   /* block rows of the component per MCU row */
+        const int lo = my0 * per, hi = my1 * per < comp[c].bcy ? my1 * per : comp[c].bcy;
+        lg.bcx[c] = comp[c].bcx;
+        lg.bcy[c] = hi > lo ? hi - lo : 0;
+        lg.blk_off[c] = comp[c].blk_off + lo * comp[c].bcx;
+        lg.wib[c] = (comp[c].width + 7) / 8;
+        lg.hib[c] = (comp[c].height + 7) / 8 - lo;
+    }
+    const int y0 = my0 * 8 * vs, y1 = my1 * 8 * vs < height ? my1 * 8 * vs : height;
+    height = y1 - y0;
+    d_raw += (ptrdiff_t)y0 * pitch;
+    LjParams prm;
+    for ( int t = 0; t < 2; t++ )
+        for ( int k = 0; k < 64; k++ ) {
+            prm.q[t][k] = raw_q[t][k];
+            prm.recip[t][k] = gj_quant_recip_libjpeg(raw_q[t][k]);
+        }
+    const dim3 grid((comp[0].bcx + TB - 1) / TB, my1 - my0);
+    const int vec = pick_vec(d_raw, (size_t)pitch);
+#define GJ_K1LJ(H, V, N)                                                                                                         \
+    do {                                                                                                                         \
+        using S = LjShape<H, V, N>;                                                                                              \
+        if ( vec == 4 )                                                                                                          \
+            gj_launch_pdl(k_fdct_libjpeg<H, V, N, 4>, grid, dim3(S::NTS), S::SMEM, stream, d_raw, width, height, (size_t)pitch, d_coef, \
+                          d_nzmask, lg, prm);                                                                                    \
+        else                                                                                                                     \
+            gj_launch_pdl(k_fdct_libjpeg<H, V, N, 1>, grid, dim3(S::NTS), S::SMEM, stream, d_raw, width, height, (size_t)pitch, d_coef, \
+                          d_nzmask, lg, prm);                                                                                    \
+    } while ( 0 )
+    if ( comp_count == 1 ) GJ_K1LJ(1, 1, 1);
+    else if ( hs == 1 && vs == 1 ) GJ_K1LJ(1, 1, 3);
+    else if ( hs == 2 && vs == 1 ) GJ_K1LJ(2, 1, 3);
+    else if ( hs == 2 && vs == 2 ) GJ_K1LJ(2, 2, 3);
+    else if ( hs == 1 && vs == 2 ) GJ_K1LJ(1, 2, 3);
+    else return -1;
+#undef GJ_K1LJ
+    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+extern "C" int gj_launch_fdct_libjpeg(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
+                                      const struct gj_comp_geo* comp, int comp_count, const uint8_t raw_q[2][64], gj_stream_t stream)
+{
+    const int vs = comp[0].vs > 0 ? comp[0].vs : 1;
+    return gj_launch_fdct_libjpeg_rows(d_raw, width, height, pitch, d_coef, d_nzmask, comp, comp_count, 0, (comp[0].bcy + vs - 1) / vs,
+                                       raw_q, stream);
 }
 
 extern "C" int gj_launch_idct_rgb_ss_rows(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], int my0, int my1,

@@ -609,6 +609,98 @@ GJ_HD void gj_ycc_rgb_libjpeg(int y, int cb, int cr, int& r, int& g, int& b)
 }
 
 /* ------------------------------------------------------------------------------------------- */
+/* enc_opt_writer=libjpeg: the coefficients libjpeg-turbo's jpeg_write_scanlines quantises after jpeg_set_defaults +            */
+/* jpeg_set_quality (jccolor's rgb_ycc_convert, jcsample's downsamplers, JDCT_ISLOW, jcdctmgr's quantiser)                      */
+
+/* jccolor.c's rgb_ycc_convert (its tables spelled out, SCALEBITS 16): every result is 0..255 without a clamp */
+GJ_HD void gj_rgb_ycc_libjpeg(int r, int g, int b, int& y, int& cb, int& cr)
+{
+    y = (19595 * r + 38470 * g + 7471 * b + 32768) >> 16;
+    cb = (-11059 * r - 21709 * g + 32768 * b + (128 << 16) + 32767) >> 16;
+    cr = (32768 * r - 27439 * g - 5329 * b + (128 << 16) + 32767) >> 16;
+}
+
+/* jcsample.c's downsamplers of a component with rh x rv times fewer samples, for output column cx: a, b the two samples of the
+ * upper (or only) row, c, d those of the lower row.  h2v2_downsample (sum + 1 + (cx & 1)) >> 2, h2v1_downsample
+ * (a + b + (cx & 1)) >> 1, int_downsample of 1x2 (a + c + 1) >> 1; 1x1 copies. */
+GJ_HD int gj_down_libjpeg(int rh, int rv, int cx, int a, int b, int c, int d)
+{
+    if ( rh == 2 && rv == 2 ) return (a + b + c + d + 1 + (cx & 1)) >> 2;
+    if ( rh == 2 ) return (a + b + (cx & 1)) >> 1;
+    if ( rv == 2 ) return (a + c + 1) >> 1;
+    return a;
+}
+
+/* One 1-D pass of jfdctint.c's jpeg_fdct_islow (CONST_BITS 13, PASS1_BITS 2) on d[0..7]: outputs 0 and 4 shifted by `even`
+ * (left by 2 in the row pass, DESCALE by 2 in the column pass: even = -2), the others DESCALEd by `odd` (11, then 15) */
+GJ_HD void gj_fislow1(int (&d)[8], int even, int odd)
+{
+    const int t0 = d[0] + d[7], t7 = d[0] - d[7], t1 = d[1] + d[6], t6 = d[1] - d[6];
+    const int t2 = d[2] + d[5], t5 = d[2] - d[5], t3 = d[3] + d[4], t4 = d[3] - d[4];
+    const int t10 = t0 + t3, t13 = t0 - t3, t11 = t1 + t2, t12 = t1 - t2;
+    const int rnd = 1 << (odd - 1);
+    if ( even > 0 ) {
+        d[0] = (t10 + t11) << even;
+        d[4] = (t10 - t11) << even;
+    }
+    else {
+        d[0] = (t10 + t11 + (1 << (-even - 1))) >> -even;
+        d[4] = (t10 - t11 + (1 << (-even - 1))) >> -even;
+    }
+    const int z1e = (t12 + t13) * 4433;
+    d[2] = (z1e + t13 * 6270 + rnd) >> odd;
+    d[6] = (z1e - t12 * 15137 + rnd) >> odd;
+    const int z1 = (t4 + t7) * -7373, z2 = (t5 + t6) * -20995;
+    const int z5 = (t4 + t6 + t5 + t7) * 9633;
+    const int z3 = (t4 + t6) * -16069 + z5, z4 = (t5 + t7) * -3196 + z5;
+    d[7] = (t4 * 2446 + z1 + z3 + rnd) >> odd;
+    d[5] = (t5 * 16819 + z2 + z4 + rnd) >> odd;
+    d[3] = (t6 * 25172 + z2 + z3 + rnd) >> odd;
+    d[1] = (t7 * 12299 + z1 + z4 + rnd) >> odd;
+}
+/* jpeg_fdct_islow on one block in place: in, the samples minus 128, row-major; out, 8x the DCT in natural order (|v| < 2^15) */
+GJ_HD void gj_fdct_islow_block(int (&v)[64])
+{
+#pragma unroll
+    for ( int r = 0; r < 8; r++ ) {
+        int d[8];
+#pragma unroll
+        for ( int i = 0; i < 8; i++ )
+            d[i] = v[8 * r + i];
+        gj_fislow1(d, 2, 11);
+#pragma unroll
+        for ( int i = 0; i < 8; i++ )
+            v[8 * r + i] = d[i];
+    }
+#pragma unroll
+    for ( int c = 0; c < 8; c++ ) {
+        int d[8];
+#pragma unroll
+        for ( int i = 0; i < 8; i++ )
+            d[i] = v[8 * i + c];
+        gj_fislow1(d, -2, 15);
+#pragma unroll
+        for ( int i = 0; i < 8; i++ )
+            v[8 * i + c] = d[i];
+    }
+}
+
+/* jcdctmgr.c's quantiser for the ISLOW DCT: divisor 8 q, sign(x) * ((|x| + 4 q) / (8 q)).  The division is a multiply by
+ * recip = floor((2^32 - 1) / (8 q)) + 1 and a high-half shift: 8 q * recip lies in [2^32, 2^32 + 8 q), so the product is exact
+ * for every n = |x| + 4 q with n * (8 q - 1) < 2^32 -- |x| < 2^15 and q <= 255 are far inside (tests check every pair). */
+GJ_HD uint32_t gj_quant_recip_libjpeg(int q) { return 0xFFFFFFFFu / (8u * (uint32_t)q) + 1u; }
+GJ_HD int gj_quant_libjpeg(int x, int q, uint32_t recip)
+{
+    const uint32_t n = (uint32_t)(x < 0 ? -x : x) + 4u * (uint32_t)q;
+#if defined(__CUDA_ARCH__)
+    const int m = (int)__umulhi(n, recip);
+#else
+    const int m = (int)(((uint64_t)n * recip) >> 32);
+#endif
+    return x < 0 ? -m : m;
+}
+
+/* ------------------------------------------------------------------------------------------- */
 /* Huffman helpers                                                                               */
 
 /* number of significant bits of |v| (JPEG "category")  [ref: src/gpujpeg_huffman_cpu_encoder.c:159-164] */

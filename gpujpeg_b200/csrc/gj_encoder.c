@@ -49,6 +49,8 @@ struct gpujpeg_encoder {
     struct gj_dev_enc_tables h_tab;            /* host copy (K1 takes it by value) */
     struct gj_dev_enc_tables* d_tab;           /* device copy (K2 LUTs) */
     int huff_optimized;                        /* enc_opt_huffman=optimized: tables fitted to every frame */
+    int writer_libjpeg;                        /* enc_opt_writer=libjpeg: libjpeg-turbo's coefficients and header */
+    int writer_mode;                           /* the writer the geometry and header were set up for */
     int spec_custom;                           /* spec / LUTs / header hold fitted tables, not Annex K */
     uint64_t* d_counts;                        /* [2][2][256] symbol counts of the statistics kernel */
     uint64_t* h_counts;                        /* pinned copy */
@@ -247,7 +249,7 @@ static int grow(void** p, size_t* have, size_t want)
  *   GJ_IN_GENERIC  any of those pixel formats in GPUJPEG_RGB / _YCBCR_BT601 / _YCBCR_BT601_256LVLS / _YCBCR_BT709 with any of
  *                  the four samplings: one extra pass converts to the JPEG's component planes (gj_convert.cu), then
  *                  the sample kernel runs on the planes */
-enum { GJ_IN_UNSUPPORTED = 0, GJ_IN_RGB = 1, GJ_IN_SAMPLES = 2, GJ_IN_GENERIC = 3 };
+enum { GJ_IN_UNSUPPORTED = 0, GJ_IN_RGB = 1, GJ_IN_SAMPLES = 2, GJ_IN_GENERIC = 3, GJ_IN_LIBJPEG = 4 };
 
 static int params_supported(const struct gpujpeg_parameters* p, const struct gpujpeg_image_parameters* pi)
 {
@@ -333,10 +335,41 @@ static int params_supported(const struct gpujpeg_parameters* p, const struct gpu
     return GJ_IN_SAMPLES;
 }
 
+/* enc_opt_writer=libjpeg takes what libjpeg-turbo's jpeg_write_scanlines takes with jpeg_set_defaults: RGB 444-u8-p012 into an
+ * interleaved YCbCr JFIF frame at 4:4:4 / 4:2:2 / 4:2:0 / 4:4:0, or GPUJPEG_U8 samples into a grey frame; the header libjpeg
+ * writes, so nothing that changes it.  Checked before anything of the encoder changes: a refused frame leaves it as it was. */
+static int libjpeg_supported(const struct gpujpeg_encoder* e, const struct gpujpeg_parameters* p, const struct gpujpeg_image_parameters* pi)
+{
+    const char* why = NULL;
+    if ( p->color_space_internal != GPUJPEG_YCBCR_BT601_256LVLS ) why = "an internal colour space other than YCbCr JPEG";
+    else if ( p->comp_count == 3 ) {
+        if ( pi->pixel_format != GPUJPEG_444_U8_P012 || pi->color_space != GPUJPEG_RGB ) why = "input other than RGB 444-u8-p012";
+        else if ( !p->interleaved ) why = "a non-interleaved colour frame";
+    }
+    else if ( p->comp_count == 1 ) {
+        if ( pi->pixel_format != GPUJPEG_U8 || pi->color_space == GPUJPEG_YCBCR_BT601 || pi->color_space == GPUJPEG_YCBCR_BT709 )
+            why = "grey input other than full-range GPUJPEG_U8";
+    }
+    else why = "a component count other than 1 or 3";
+    if ( !why && (e->flipped || e->channel_remap) ) why = "enc_opt_flipped / enc_opt_channel_remap";
+    if ( !why && p->segment_info ) why = "segment info";
+    if ( !why && ((e->header_type != GPUJPEG_HEADER_DEFAULT && e->header_type != GPUJPEG_HEADER_JFIF) || e->extras.exif_tags ||
+                  e->extras.metadata.vals[GPUJPEG_METADATA_ORIENTATION].set) )
+        why = "a header other than JFIF (enc_hdr, enc_exif_tag, enc_metadata)";
+    if ( why ) {
+        GJ_ERR(GPUJPEG_ENC_OPT_WRITER "=" GPUJPEG_ENC_WRITER_VAL_LIBJPEG " does not take %s.\n", why);
+        return 0;
+    }
+    return 1;
+}
+
 /* K1 for the coder's geometry: the 4:4:4 kernel or the chroma-subsampling template instance */
 static int launch_k1(struct gpujpeg_encoder* e, const uint8_t* d_raw)
 {
     const struct gj_geometry* g = &e->geo;
+    if ( e->input_mode == GJ_IN_LIBJPEG )
+        return gj_launch_fdct_libjpeg(d_raw, g->width, g->height, g->comp_count == 1 ? (int)e->raw.comp[0].pitch : g->pitch, e->d_coef,
+                                      e->d_nzmask, g->comp, g->comp_count, (const uint8_t(*)[64])e->raw_q, e->stream);
     if ( e->input_mode == GJ_IN_SAMPLES )
         return gj_launch_fdct_samples(d_raw, &e->raw, e->d_coef, e->d_nzmask, g->comp, g->comp_count, g->lay.comp_tbl, &e->h_tab,
                                       e->stream);
@@ -367,11 +400,12 @@ static int launch_k1(struct gpujpeg_encoder* e, const uint8_t* d_raw)
 
 static void fill_huff_args(const struct gpujpeg_encoder* e, struct gj_huff_enc_args* ha);
 
-/* The stripe pipeline applies to what the fused RGB kernels take as it comes: no flip, no channel remap. */
+/* The stripe pipeline applies to what the fused RGB kernels (either writer's) take as it comes: no flip, no channel remap. */
 static int stripes_usable(struct gpujpeg_encoder* e)
 {
     const struct gj_geometry* g = &e->geo;
-    if ( e->input_mode != GJ_IN_RGB || e->flipped || e->channel_remap ) return 0;
+    if ( !(e->input_mode == GJ_IN_RGB || (e->input_mode == GJ_IN_LIBJPEG && g->comp_count == 3)) || e->flipped || e->channel_remap )
+        return 0;
     if ( e->stripes == 0 ) {
         const char* v = getenv("GPUJPEG_B200_STRIPES");
         const char* m = getenv("GPUJPEG_B200_STRIPE_MIN_BYTES");
@@ -422,7 +456,10 @@ static int encode_striped(struct gpujpeg_encoder* e, const uint8_t* h_image, int
         if ( gj_cuda_memcpy_h2d_async(e->d_raw + off, h_image + off, bytes, e->copy_stream) ||
              gj_cuda_event_record(e->ev_stripe[i], e->copy_stream) || gj_cuda_stream_wait_event(e->stream, e->ev_stripe[i]) )
             return -1;
-        const int rc = g->lay.simple ? gj_launch_fdct_rgb444_rows(e->d_raw, g->width, g->height, g->pitch, e->d_coef, e->d_nzmask, g->bcx,
+        const int rc = e->input_mode == GJ_IN_LIBJPEG
+                           ? gj_launch_fdct_libjpeg_rows(e->d_raw, g->width, g->height, g->pitch, e->d_coef, e->d_nzmask, g->comp, 3, my0, my1,
+                                                         (const uint8_t(*)[64])e->raw_q, e->stream)
+                       : g->lay.simple ? gj_launch_fdct_rgb444_rows(e->d_raw, g->width, g->height, g->pitch, e->d_coef, e->d_nzmask, g->bcx,
                                                                   g->bcy, my0, my1, &e->h_tab, e->stream)
                                      : gj_launch_fdct_rgb_ss_rows(e->d_raw, g->width, g->height, g->pitch, e->d_coef, e->d_nzmask, g->comp,
                                                                   my0, my1, &e->h_tab, e->stream);
@@ -547,7 +584,8 @@ static int encoder_init_image(struct gpujpeg_encoder* e, const struct gpujpeg_pa
 {
     gj_geometry_init(&e->geo, p, pi);
     e->geo.stream_cap += e->extras.com_size;
-    e->input_mode = e->coef_input ? GJ_IN_UNSUPPORTED : params_supported(p, pi);
+    e->input_mode = e->coef_input ? GJ_IN_UNSUPPORTED : e->writer_libjpeg ? GJ_IN_LIBJPEG : params_supported(p, pi);
+    e->writer_mode = e->writer_libjpeg;
     /* the flip acts on the component planes, padding included [ref: src/gpujpeg_preprocessor.cu:474-485]: in general only the
      * pass that has planes can do it.  When no component is subsampled vertically and the height has no padding, flipping
      * the planes is flipping the image rows, and the fused kernel does that by reading the rows backwards (launch_k1).
@@ -910,7 +948,7 @@ int gpujpeg_encoder_encode(struct gpujpeg_encoder* e, const struct gpujpeg_param
     struct gpujpeg_parameters a = adjust_params(e, param, param_image, img_changed);
     const int stats = a.perf_stats || a.verbose >= GPUJPEG_LL_STATUS;
     const double t_begin = stats ? gpujpeg_get_time() : 0.0;
-    if ( !params_supported(&a, param_image) ) return GPUJPEG_ERROR;
+    if ( !params_supported(&a, param_image) || (e->writer_libjpeg && !libjpeg_supported(e, &a, param_image)) ) return GPUJPEG_ERROR;
 
     /* quantisation tables follow the quality [ref: src/gpujpeg_encoder.c:372-380] */
     int tables_dirty = 0;
@@ -926,7 +964,7 @@ int gpujpeg_encoder_encode(struct gpujpeg_encoder* e, const struct gpujpeg_param
     e->counts_valid = 0;
     int geometry_dirty = 0;
     if ( img_changed || !same_param(&e->param, &a) || e->out_is_pinned != e->out_pinned || !e->out ||
-         (e->flipped != 0) != e->flip_mode ) {
+         (e->flipped != 0) != e->flip_mode || e->writer_libjpeg != e->writer_mode ) {
         if ( encoder_init_image(e, &a, param_image) ) return GPUJPEG_ERROR;
         geometry_dirty = 1;
     }
@@ -1185,6 +1223,17 @@ int gpujpeg_encoder_set_option(struct gpujpeg_encoder* encoder, const char* opt,
         }
         return GPUJPEG_NOERR;
     }
+    if ( strcmp(opt, GPUJPEG_ENC_OPT_WRITER) == 0 ) {   /* extension: whose file the encoder writes */
+        if ( strcmp(val, GPUJPEG_ENC_WRITER_VAL_GPUJPEG) == 0 ) encoder->writer_libjpeg = 0;
+        else if ( strcmp(val, GPUJPEG_ENC_WRITER_VAL_LIBJPEG) == 0 ) encoder->writer_libjpeg = 1;
+        else {
+            GJ_ERR("Unknown encoder writer: %s\n", val);
+            return GPUJPEG_ERROR;
+        }
+        encoder->extras.libjpeg = encoder->writer_libjpeg;
+        encoder->extras_dirty = 1;
+        return GPUJPEG_NOERR;
+    }
     GJ_ERR("Invalid encoder option: %s!\n", opt);
     return GPUJPEG_ERROR;
 }
@@ -1203,10 +1252,12 @@ void gpujpeg_encoder_print_options(void)
            "\t\t'210' for GBR; special placeholders 'F' and 'Z' to set a channel to all-ones or all-zeros\n");
     printf("\t" GPUJPEG_ENC_OPT_HUFFMAN "=[" GPUJPEG_ENC_HUFFMAN_VAL_STANDARD "|" GPUJPEG_ENC_HUFFMAN_VAL_OPTIMIZED
            "] - Huffman tables of T.81 Annex K (default) or fitted to every frame\n");
+    printf("\t" GPUJPEG_ENC_OPT_WRITER "=[" GPUJPEG_ENC_WRITER_VAL_GPUJPEG "|" GPUJPEG_ENC_WRITER_VAL_LIBJPEG
+           "] - this library's stream (default) or the file libjpeg-turbo writes with its defaults\n");
 }
 
 /* ---- extension: re-run the GPU stages of the last configured frame on device-resident data ----
- * stage_mask bit 0 = K1 (colour+FDCT+quant), bit 3 = the symbol statistics of enc_opt_huffman=optimized (kernel alone),
+ * stage_mask bit 0 = K1 (colour+FDCT+quant, the kernel of the writer chosen), bit 3 = the symbol statistics of enc_opt_huffman=optimized (kernel alone),
  * bit 1 = K2 (Huffman encode + scan assembly, with the tables the last gpujpeg_encoder_encode chose).  Nothing is
  * copied to or from the host and nothing is synchronised: the caller times the stream with CUDA events.
  * d_raw == NULL re-uses the device copy of the last host image.  Used by bench.py for the

@@ -250,6 +250,7 @@ struct gj_header_extras {
     /* whole COM segments (markers included) that replace the writer's own comments; NULL: the writer's */
     const uint8_t* com;
     size_t com_size;
+    int libjpeg;   /* enc_opt_writer=libjpeg: the header libjpeg-turbo writes for a JFIF frame (gj_write_header) */
 };
 #define GJ_HEADER_BASE_CAP 1024   /* bytes a header needs at most without user Exif tags */
 size_t gj_write_header(uint8_t* out, const struct gpujpeg_parameters* param,
@@ -385,6 +386,15 @@ int gj_launch_idct_rgb444_rows(const int16_t* d_coef, const uint8_t* d_cext, int
 int gj_launch_fdct_rgb_ss_rows(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
                                const struct gj_comp_geo comp[3], int my0, int my1, const struct gj_dev_enc_tables* h_tables,
                                gj_stream_t stream);
+/* enc_opt_writer=libjpeg: libjpeg-turbo's colour conversion, downsampling, ISLOW FDCT and quantiser (raw_q: the DQT tables,
+ * zig-zag), with its edge replication and the dummy blocks of interleaved MCUs.  comp_count 3: RGB u8 interleaved, luminance
+ * 1x1, 2x1, 2x2 or 1x2 and chrominance 1x1; comp_count 1: grey u8.  pitch: bytes per image row.  The _rows variant transforms
+ * MCU rows [my0, my1) only (an MCU row = 8 * comp[0].vs image rows). */
+int gj_launch_fdct_libjpeg(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
+                           const struct gj_comp_geo* comp, int comp_count, const uint8_t raw_q[2][64], gj_stream_t stream);
+int gj_launch_fdct_libjpeg_rows(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
+                                const struct gj_comp_geo* comp, int comp_count, int my0, int my1, const uint8_t raw_q[2][64],
+                                gj_stream_t stream);
 int gj_launch_idct_rgb_ss_rows(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], int my0, int my1,
                                const int comp_tq[3], uint8_t* d_raw, int width, int height, int pitch, int idct_flavour,
                                int coef_dequantized, const struct gj_dev_dec_tables* h_tables, gj_stream_t stream);

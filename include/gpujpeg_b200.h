@@ -383,6 +383,20 @@ GPUJPEG_API int gpujpeg_encoder_suggest_restart_interval(const struct gpujpeg_im
 #define GPUJPEG_ENC_OPT_HUFFMAN "enc_opt_huffman"
 #define GPUJPEG_ENC_HUFFMAN_VAL_STANDARD "standard"
 #define GPUJPEG_ENC_HUFFMAN_VAL_OPTIMIZED "optimized"
+/* extension: whose file the encoder writes.  "gpujpeg" (default): this library's stream (float AAN FDCT, point-sampled chroma, a
+ * COM segment and a DRI marker).  "libjpeg": the file libjpeg-turbo's jpeg_write_scanlines writes after jpeg_set_defaults +
+ * jpeg_set_quality(quality, TRUE) -- what PIL's Image.save(quality=q, subsampling=s, optimize=o, restart_marker_blocks=r) writes,
+ * byte for byte: its integer colour conversion, chroma downsampling and edge replication, the ISLOW FDCT and its quantiser, the
+ * DC of the dummy blocks of interleaved MCUs, and its header (JFIF 1.01 aspect 1:1, DQT, SOF0, DHT, DRI only for a non-zero
+ * interval, no COM).  enc_opt_huffman=optimized corresponds to optimize=True; restart_interval counts MCUs as libjpeg's (0: no
+ * restart markers, libjpeg's default; RESTART_AUTO: the suggested interval).  Input: GPUJPEG_RGB 444-u8-p012 (host or device,
+ * any row padding) into an interleaved YCbCr frame at 4:4:4, 4:2:2, 4:2:0 or 4:4:0, or GPUJPEG_U8 into a grey frame.  Refused
+ * with a message, the encoder staying usable: other pixel formats, input or internal colour spaces, four components, a
+ * non-interleaved colour frame, enc_opt_flipped, enc_opt_channel_remap, segment_info, enc_hdr other than the default or JFIF,
+ * enc_exif_tag and enc_metadata.  The gpujpegx_batch_* workers do not offer it. */
+#define GPUJPEG_ENC_OPT_WRITER "enc_opt_writer"
+#define GPUJPEG_ENC_WRITER_VAL_GPUJPEG "gpujpeg"
+#define GPUJPEG_ENC_WRITER_VAL_LIBJPEG "libjpeg"
 GPUJPEG_API int gpujpeg_encoder_set_option(struct gpujpeg_encoder* encoder, const char* opt, const char* val);
 GPUJPEG_API void gpujpeg_encoder_print_options(void);
 GPUJPEG_API int gpujpeg_encoder_destroy(struct gpujpeg_encoder* encoder);
