@@ -721,6 +721,93 @@ GJ_HD unsigned gj_value_bits(int v, int size) { return (unsigned)(v < 0 ? v - 1 
 GJ_HD int gj_extend(int bits, int size) { return bits < (1 << (size - 1)) ? bits - (1 << size) + 1 : bits; }
 
 /* ------------------------------------------------------------------------------------------- */
+/* Huffman encoding of long restart segments (more than 40 blocks: k_huff_chunk + k_huff_stuff in gj_huffman.cu).        */
+/* A segment is cut, in coding order, into chunks of GJ_HS_CHUNK blocks, coded one CTA per chunk into a word-aligned bit   */
+/* string of its own; the segment's unstuffed bit image is the concatenation of its chunks' strings, padded with 1-bits to */
+/* a byte boundary; tiles of GJ_HS_TILE bytes of that image are byte-stuffed and placed into the stream.                  */
+#define GJ_HS_CHUNK 128   /* blocks per chunk (one thread per block); every chunk but a segment's last holds >= 256 bits */
+#define GJ_HS_TILE 8192   /* unstuffed bytes per tile (256 threads x 32 bytes) */
+
+GJ_HD int gj_hs_chunks(int blocks) { return (blocks + GJ_HS_CHUNK - 1) / GJ_HS_CHUNK; }
+/* tiles of a segment whose image holds `bits` bits (at least one: a segment has at least one block) */
+GJ_HD uint64_t gj_hs_seg_bytes(uint64_t bits) { return (bits + 7) >> 3; }
+GJ_HD uint64_t gj_hs_tiles(uint64_t bits) { return (gj_hs_seg_bytes(bits) + GJ_HS_TILE - 1) / GJ_HS_TILE; }
+
+/* bytes equal to 0xFF in w: each is followed by a stuffed zero byte in the stream */
+GJ_HD int gj_hs_ff_count(uint32_t w)
+{
+    const uint32_t t = w & (w >> 4) & 0x0F0F0F0Fu;
+    const uint32_t ff = t & (t >> 2) & 0x03030303u;
+    const uint32_t m = ff & (ff >> 1) & 0x01010101u;   /* bit 0 of every byte that is 0xFF */
+#if defined(__CUDA_ARCH__)
+    return __popc(m);
+#else
+    return __builtin_popcount(m);
+#endif
+}
+/* the first `nbytes` bytes of a big-endian word (all four for nbytes >= 4) */
+GJ_HD uint32_t gj_hs_keep(uint32_t nbytes) { return nbytes >= 4 ? 0xFFFFFFFFu : ~(0xFFFFFFFFu >> (8 * nbytes)); }
+/* stream bytes of the first `nbytes` bytes of the big-endian words w[]: every byte, plus a zero after every 0xFF */
+GJ_HD uint32_t gj_hs_stuffed_bytes(const uint32_t* w, uint32_t nbytes)
+{
+    uint32_t n = nbytes;
+    for ( uint32_t q = 0; 4 * q < nbytes; q++ )
+        n += (uint32_t)gj_hs_ff_count(w[q] & gj_hs_keep(nbytes - 4 * q));
+    return n;
+}
+
+/* The word of a segment's unstuffed image that starts at bit p (a multiple of 32), read from the chunk holding bit p: `a`
+ * its words, [o, e) its bits in the segment (o <= p < e), `next0` the first word of the chunk that follows (0 if none).
+ * Bits of `a` past e are never used, so a chunk's string need not be cleared behind its end. */
+GJ_HD uint32_t gj_hs_gather(const uint32_t* a, uint64_t o, uint64_t e, uint32_t next0, uint64_t p)
+{
+    const uint64_t off = p - o;
+    const uint32_t q = (uint32_t)(off >> 5), sh = (uint32_t)off & 31u;
+    const uint64_t nw = (e - o + 31) >> 5;
+    uint32_t w = a[q] << sh;
+    if ( sh && q + 1 < nw ) w |= a[q + 1] >> (32 - sh);
+    const uint64_t rem = e - p;   /* bits of this chunk from p on */
+    if ( rem < 32 ) w = (w & ~(0xFFFFFFFFu >> rem)) | (next0 >> rem);
+    return w;
+}
+/* the end of a segment of `bits` bits: 1-bits from `bits` to the next byte boundary [ref: src/gpujpeg_huffman_cpu_encoder.c:
+ * 115-128], applied to the word that starts at bit p (a multiple of 32) */
+GJ_HD uint32_t gj_hs_pad(uint32_t w, uint64_t p, uint64_t bits)
+{
+    const uint64_t end = (bits + 7) & ~(uint64_t)7;
+    if ( bits == end || bits >= p + 32 || end <= p ) return w;
+    const uint32_t lo = (uint32_t)(bits - p), hi = (uint32_t)(end - p);   /* 0 < hi - lo < 8, hi <= 32 */
+    return w | ((0xFFFFFFFFu >> lo) & ~(hi >= 32 ? 0u : 0xFFFFFFFFu >> hi));
+}
+/* Concatenation of chunk strings at bit offsets, as k_huff_stuff reads them: the image words [w0, w0 + n) of a segment whose
+ * k chunks end at bits e[0..k-1] (cumulative), chunk c's string at chunk[c * stride], padded at the segment's end.  Host
+ * restatement of the kernel's gather for the tests; the kernel finds the chunk of each word by a search over the same ends. */
+GJ_HD void gj_hs_image_words(const uint32_t* chunk, uint64_t stride, const uint64_t* e, int k, uint64_t w0, uint32_t n, uint32_t* out)
+{
+    int c = 0;
+    for ( uint32_t i = 0; i < n; i++ ) {
+        const uint64_t p = 32 * (w0 + i);
+        while ( c < k && e[c] <= p ) c++;
+        uint32_t w = 0;
+        if ( c < k ) w = gj_hs_gather(chunk + c * stride, c ? e[c - 1] : 0, e[c], c + 1 < k ? chunk[(c + 1) * stride] : 0u, p);
+        out[i] = gj_hs_pad(w, p, k ? e[k - 1] : 0);
+    }
+}
+/* Stream bytes around segment s (number in its scan) of a scan of `segs` segments: in front, `pre` (the scan's [APP13] SOS
+ * bytes) before its first segment; behind, RSTn after every other segment and EOI after the frame's last */
+GJ_HD uint32_t gj_hs_seg_front(int s, uint32_t pre) { return s == 0 ? pre : 0u; }
+GJ_HD uint32_t gj_hs_seg_back(int s, int segs, bool last_of_frame) { return s + 1 < segs || last_of_frame ? 2u : 0u; }
+
+/* The frame's plan: chunks per segment of `segblk` blocks, tiles per segment whose slot holds `slot_stride` bytes (a segment's
+ * image never exceeds its slot: a chunk that does not fit its part reports the overflow instead), and the status words of
+ * both look-backs */
+GJ_HD uint64_t gj_hs_tiles_per_slot(uint64_t slot_stride) { return gj_hs_tiles(slot_stride * 8); }
+GJ_HD uint64_t gj_hs_status_words(int seg_count, int segblk, uint64_t slot_stride)
+{
+    return (uint64_t)seg_count * ((uint64_t)gj_hs_chunks(segblk) + gj_hs_tiles_per_slot(slot_stride));
+}
+
+/* ------------------------------------------------------------------------------------------- */
 /* progressive Huffman decoding (T.81 G.2), one restart segment per thread: k_prog_decode         */
 
 /* Bits of one restart segment of K0's clean stream (big-endian 32-bit words, stuffing and markers removed): a 64-bit

@@ -64,8 +64,13 @@ struct gpujpeg_encoder {
     size_t slot_stride;              /* bytes per restart segment in d_tmp: starts at 48 bytes per block (photographic and noisy
                                       * content at any common quality), grows to what a frame needed when K2 reports an overflow;
                                       * the worst case (geo.slot_stride, 416 bytes per block: 648 MB for an 8K frame) is only ever
-                                      * allocated for content that needs it */
+                                      * allocated for content that needs it.  Segments on K2's chunk path (gj_huffman.cu) split
+                                      * their slot into equal parts per block, one per chunk of 128 blocks: there the DENSEST
+                                      * chunk sets the size (a photo with one noisy region can outgrow 48 bytes per block where
+                                      * the whole segment would not, and then re-runs K2 once with slots of up to 216 bytes
+                                      * per block) */
     uint32_t* d_spill; size_t d_spill_size;
+    uint64_t* d_split; size_t d_split_size;  /* status words of the long-segment path of K2 */
     uint32_t* d_seg_bytes; uint64_t* d_seg_off; int seg_alloc;
     uint8_t* d_stream; size_t d_stream_size;
     uint8_t* d_sos; size_t d_sos_size;        /* per scan: [APP13 segment-info headers] SOS header */
@@ -200,6 +205,7 @@ int gpujpeg_encoder_destroy(struct gpujpeg_encoder* e)
     gj_cuda_free(e->d_nzmask);
     gj_cuda_free(e->d_tmp);
     gj_cuda_free(e->d_spill);
+    gj_cuda_free(e->d_split);
     gj_cuda_free(e->d_seg_bytes);
     gj_cuda_free(e->d_seg_off);
     gj_cuda_free(e->d_stream);
@@ -530,6 +536,8 @@ static void fill_huff_args(const struct gpujpeg_encoder* e, struct gj_huff_enc_a
     ha->d_info_next = e->d_info + 4 * (e->info_parity ^ 1);
     ha->info_is_zero = e->info_clean;
     ha->d_tables = e->d_tab;
+    ha->d_split = e->d_split;
+    ha->split_bytes = e->d_split_size;
 }
 
 /* the symbol statistics of the frame K1 left in place (enqueued only) */
@@ -604,13 +612,15 @@ static int encoder_init_image(struct gpujpeg_encoder* e, const struct gpujpeg_pa
     if ( e->slot_stride < first_stride || e->slot_stride > g->slot_stride ) e->slot_stride = first_stride;
     size_t tmp_bytes = (size_t)g->seg_count * e->slot_stride + 256;
     /* overflow area of the per-block bit strings: 32 words per block of a short segment (packed kernel, <= 40 blocks),
-     * per lane of a warp otherwise (streaming kernel) */
+     * per lane of a warp otherwise (streaming kernel); the chunks of few long segments need status words instead */
     const int segblk = g->seg_mcu * g->lay.bpm;
     size_t spill_bytes = (size_t)g->seg_count * (segblk <= 40 ? segblk : 32) * 32 * sizeof(uint32_t);
+    const size_t split_bytes = gj_huffman_split_status_bytes(g->seg_count, segblk, g->slot_stride);
     if ( grow((void**)&e->d_coef, &e->d_coef_size, coef_bytes) ||
          grow((void**)&e->d_nzmask, &e->d_nzmask_size, g->coef_count / 64 * sizeof(uint64_t)) ||
          grow((void**)&e->d_tmp, &e->d_tmp_size, tmp_bytes) ||
          grow((void**)&e->d_spill, &e->d_spill_size, spill_bytes) ||
+         grow((void**)&e->d_split, &e->d_split_size, split_bytes) ||
          grow((void**)&e->d_stream, &e->d_stream_size, g->stream_cap + 64) ) {
         GJ_ERR("Encoder device allocation failed (%zu + %zu + %zu bytes): %s\n", coef_bytes, tmp_bytes, g->stream_cap,
                gj_cuda_last_error());

@@ -9,9 +9,14 @@
  *                   packed (sparse walk over the 64-bit non-zero mask K1 wrote next to the zig-zag ordered
  *                   coefficients); phase B, one WARP per segment, places the strings by a prefix sum over
  *                   their lengths into a shared-memory stream buffer and byte-stuffs it into the segment's slot.
- *   k_huff_encode   segments of any length (even restart_interval = 0): one WARP per segment, one LANE per block,
- *                   the same steps per round of 32 blocks, streaming through the 2 KB buffer.
- *   k_huff_place    final byte offsets of the segments by a decoupled look-back over the CTAs' byte counts
+ *   k_huff_encode   segments of a few hundred blocks (see HE_WARP_MAXBLK): one WARP per segment, one LANE per block,
+ *                   rounds of 32 blocks streaming through a 2 KB buffer.
+ *   k_huff_chunk    longer segments (restart_interval = 0 included), parallel over blocks whatever the interval: a CTA per
+ *                   chunk of 128 blocks, one THREAD per block, the chunk's string in its part of the segment's slot and its
+ *                   bit offset in the segment by a decoupled look-back;
+ *   k_huff_stuff    then tiles of 8 KB of each segment's unstuffed image, gathered from the chunks, byte-stuffed and written
+ *                   straight to their place in the stream (offsets by a look-back over the tiles, markers included).
+ *   k_huff_place    (short segments) final byte offsets of the segments by a decoupled look-back over the CTAs' byte counts
  *                   (deterministic, unlike the reference's atomicAdd compaction), then every segment to its final
  *                   place with its RSTn marker, the SOS headers prepared by the host writer and EOI: the device
  *                   buffer then holds the finished scan data and the host does a single D2H copy.
@@ -134,6 +139,56 @@ constexpr int HE_SPILL = 32;   // further words per lane in global memory: an 8x
                                // 54 words in total (64 x (16-bit code + 11 value bits))
 constexpr int HE_HEAD = 12;    // words per lane holding the first 16 coefficients of its block (8 used; the 48-byte
                                // stride keeps the lanes' 16-byte stores on distinct bank groups)
+/* One block's bit string [ref: src/gpujpeg_huffman_cpu_encoder.c:140-190]: the DC difference to `pred`, then every non-zero
+ * AC coefficient -- the set bits of the block's non-zero mask `nz`, which K1 wrote next to the zig-zag ordered coefficients --
+ * with the zero runs in front of it (ZRL per 16), EOB unless coefficient 63 is non-zero.  head16: the block's first 16
+ * coefficients, staged in shared memory; blk: the block; s_dc / s_ac: the code tables in shared memory, class `tbl`.  Every
+ * complete 32-bit word goes to put(i, word), then the left-aligned remainder (low bits zero); returns the length in bits. */
+template <class Put>
+__device__ __forceinline__ int code_block(int dc, int pred, uint64_t nz, const int16_t* head16, const int16_t* __restrict__ blk,
+                                          const uint32_t (*s_ac)[256], const uint32_t (*s_dc)[16], int tbl, Put put)
+{
+    uint64_t acc = 0;
+    int nb = 0, wi = 0;
+    auto emit = [&](int len, uint32_t bits) {   // (the length first, as the shifts use it first)
+        acc = (acc << len) | (uint64_t)bits;
+        nb += len;
+        if ( nb >= 32 ) {
+            put(wi, (uint32_t)(acc >> (nb - 32)));
+            wi++;
+            nb -= 32;
+        }
+    };
+    const int diff = dc - pred;
+    const int dcat = gj_category(diff);
+    const uint32_t de = s_dc[tbl][dcat];
+    emit((int)(de & 31u) + dcat, ((de >> 5) << dcat) | (dcat ? gj_value_bits(diff, dcat) : 0u));
+    uint32_t mlo = (uint32_t)nz & ~1u, mhi = (uint32_t)(nz >> 32);
+    int last = 0;
+    const uint32_t zrl = s_ac[tbl][0xF0];
+    while ( mlo | mhi ) {
+        int k;
+        if ( mlo ) { k = __ffs((int)mlo) - 1; mlo &= mlo - 1; }
+        else { k = 32 + __ffs((int)mhi) - 1; mhi &= mhi - 1; }
+        int run = k - last - 1;
+        last = k;
+        const int v = k < 16 ? (int)head16[k] : (int)__ldg(blk + k);
+        const int size = gj_category(v);
+        while ( run > 15 ) {
+            emit((int)(zrl & 31u), zrl >> 5);
+            run -= 16;
+        }
+        const uint32_t e = s_ac[tbl][(run << 4) | size];
+        emit((int)(e & 31u) + size, ((e >> 5) << size) | gj_value_bits(v, size));
+    }
+    if ( last < 63 ) {
+        const uint32_t e = s_ac[tbl][0];
+        emit((int)(e & 31u), e >> 5);
+    }
+    if ( nb ) put(wi, (uint32_t)(acc << (32 - nb)));
+    return 32 * wi + nb;
+}
+
 constexpr int HE_SMEM = (2 * 256 + 2 * 16 + HE_WARPS * HE_WORDS + HE_WARPS * 32 * HE_PRIV + HE_WARPS * 32 * HE_HEAD) * 4;
 
 /* One WARP per restart segment, one LANE per 8x8 block, ONE pass per block:
@@ -237,53 +292,10 @@ k_huff_encode(const int16_t* __restrict__ coef, const uint64_t* __restrict__ nzm
         /* ---- 1. the block's bit string, into the lane's private words ---- */
         int len = 0;   // total bits of this block
         if ( active ) {
-            uint64_t acc = 0;
-            int nb = 0, wi = 0;
-#define GJ_PUT(bits_, len_)                                        \
-    do {                                                           \
-        acc = (acc << (len_)) | (uint64_t)(bits_);                 \
-        nb += (len_);                                              \
-        if ( nb >= 32 ) {                                          \
-            const uint32_t w_ = (uint32_t)(acc >> (nb - 32));      \
-            if ( wi < HE_PRIV ) priv[wi] = w_;                     \
-            else spill[wi - HE_PRIV] = w_;                         \
-            wi++;                                                  \
-            nb -= 32;                                              \
-        }                                                          \
-    } while ( 0 )
-            const int diff = dc - pred;
-            const int dcat = gj_category(diff);
-            const uint32_t de = s_dc[tbl][dcat];
-            GJ_PUT(((de >> 5) << dcat) | (dcat ? gj_value_bits(diff, dcat) : 0u), (int)(de & 31u) + dcat);
-            uint32_t mlo = (uint32_t)nz & ~1u, mhi = (uint32_t)(nz >> 32);
-            int last = 0;
-            const uint32_t zrl = s_ac[tbl][0xF0];
-            while ( mlo | mhi ) {
-                int k;
-                if ( mlo ) { k = __ffs((int)mlo) - 1; mlo &= mlo - 1; }
-                else { k = 32 + __ffs((int)mhi) - 1; mhi &= mhi - 1; }
-                int run = k - last - 1;
-                last = k;
-                const int v = k < 16 ? (int)head16[k] : (int)__ldg(blk + k);
-                const int size = gj_category(v);
-                while ( run > 15 ) {
-                    GJ_PUT(zrl >> 5, (int)(zrl & 31u));
-                    run -= 16;
-                }
-                const uint32_t e = s_ac[tbl][(run << 4) | size];
-                GJ_PUT(((e >> 5) << size) | gj_value_bits(v, size), (int)(e & 31u) + size);
-            }
-            if ( last < 63 ) {
-                const uint32_t e = s_ac[tbl][0];
-                GJ_PUT(e >> 5, (int)(e & 31u));
-            }
-#undef GJ_PUT
-            if ( nb ) {   // left-aligned tail, low bits zero
-                const uint32_t w_ = (uint32_t)(acc << (32 - nb));
-                if ( wi < HE_PRIV ) priv[wi] = w_;
-                else spill[wi - HE_PRIV] = w_;
-            }
-            len = 32 * wi + nb;
+            len = code_block(dc, pred, nz, head16, blk, s_ac, s_dc, tbl, [&](int wi, uint32_t w) {
+                if ( wi < HE_PRIV ) priv[wi] = w;
+                else spill[wi - HE_PRIV] = w;
+            });
         }
         const int incl = warp_incl_scan(len, lane);
         const int excl = incl - len;
@@ -362,7 +374,7 @@ k_huff_encode(const int16_t* __restrict__ coef, const uint64_t* __restrict__ nzm
  *   phase A  all blocks of the CTA's segments, densely packed onto the threads (288 blocks = 9 full warp rounds
  *            instead of 16 half-empty ones): each thread builds its block's bit string in shared memory;
  *   phase B  one warp per segment: prefix sum over the string lengths, placement into the stream buffer, byte
- *            stuffing -- steps 2-4 of k_huff_encode, unchanged. */
+ *            stuffing. */
 constexpr int HP_MAXBLK = 40;   // blocks per segment the packed kernel takes
 constexpr int HP_THREADS_MAX = HE_WARPS * HP_MAXBLK;   // one thread per block of the CTA's segments (rounded to warps)
 /* the per-thread coefficient heads (phase A) live in the stream buffers (phase B): 8 x 512 words >= 256 x 12 words */
@@ -448,53 +460,10 @@ k_huff_encode_packed(const int16_t* __restrict__ coef, const uint64_t* __restric
             const int dc = (int)(short)(ha.x & 0xFFFFu);
             uint32_t* priv = s_priv + lb * HE_PRIV;
             uint32_t* spill = spill_all + ((size_t)g * segblk + j) * HE_SPILL;
-            uint64_t acc = 0;
-            int nb = 0, wi = 0;
-#define GJ_PUT(bits_, len_)                                        \
-    do {                                                           \
-        acc = (acc << (len_)) | (uint64_t)(bits_);                 \
-        nb += (len_);                                              \
-        if ( nb >= 32 ) {                                          \
-            const uint32_t w_ = (uint32_t)(acc >> (nb - 32));      \
-            if ( wi < HE_PRIV ) priv[wi] = w_;                     \
-            else spill[wi - HE_PRIV] = w_;                         \
-            wi++;                                                  \
-            nb -= 32;                                              \
-        }                                                          \
-    } while ( 0 )
-            const int diff = dc - pred;
-            const int dcat = gj_category(diff);
-            const uint32_t de = s_dc[tbl][dcat];
-            GJ_PUT(((de >> 5) << dcat) | (dcat ? gj_value_bits(diff, dcat) : 0u), (int)(de & 31u) + dcat);
-            uint32_t mlo = (uint32_t)nz & ~1u, mhi = (uint32_t)(nz >> 32);
-            int last = 0;
-            const uint32_t zrl = s_ac[tbl][0xF0];
-            while ( mlo | mhi ) {
-                int k;
-                if ( mlo ) { k = __ffs((int)mlo) - 1; mlo &= mlo - 1; }
-                else { k = 32 + __ffs((int)mhi) - 1; mhi &= mhi - 1; }
-                int run = k - last - 1;
-                last = k;
-                const int v = k < 16 ? (int)head16[k] : (int)__ldg(blk + k);
-                const int size = gj_category(v);
-                while ( run > 15 ) {
-                    GJ_PUT(zrl >> 5, (int)(zrl & 31u));
-                    run -= 16;
-                }
-                const uint32_t e = s_ac[tbl][(run << 4) | size];
-                GJ_PUT(((e >> 5) << size) | gj_value_bits(v, size), (int)(e & 31u) + size);
-            }
-            if ( last < 63 ) {
-                const uint32_t e = s_ac[tbl][0];
-                GJ_PUT(e >> 5, (int)(e & 31u));
-            }
-#undef GJ_PUT
-            if ( nb ) {   // left-aligned tail, low bits zero
-                const uint32_t w_ = (uint32_t)(acc << (32 - nb));
-                if ( wi < HE_PRIV ) priv[wi] = w_;
-                else spill[wi - HE_PRIV] = w_;
-            }
-            s_len[lb] = (uint32_t)(32 * wi + nb);
+            s_len[lb] = (uint32_t)code_block(dc, pred, nz, head16, blk, s_ac, s_dc, tbl, [&](int wi, uint32_t w) {
+                if ( wi < HE_PRIV ) priv[wi] = w;
+                else spill[wi - HE_PRIV] = w;
+            });
         }
     }
     __syncthreads();
@@ -552,7 +521,7 @@ k_huff_encode_packed(const int16_t* __restrict__ coef, const uint64_t* __restric
             __syncwarp();
         }
         else {
-            /* dense content: stream the segment through the buffer in rounds, as k_huff_encode does */
+            /* dense content: stream the segment through the buffer in rounds */
             for ( int base = 0; base < nblocks; base += 32 ) {
                 const int j = base + lane;
                 const bool active = j < nblocks;
@@ -766,6 +735,318 @@ k_huff_place(const uint8_t* __restrict__ tmp, size_t slot_stride, const uint32_t
             dst[n] = 0xFF;
             dst[n + 1] = 0xD9;
         }
+    }
+}
+
+/* ------------------------------------------------------------------------------------------- */
+/* Long segments (more than HP_MAXBLK blocks, restart_interval = 0 included): parallel over blocks whatever the interval.
+ *   k_huff_chunk  one CTA per chunk of GJ_HS_CHUNK blocks of a segment (coding order), one THREAD per block: the block's bit
+ *                 string (code_block, as phase A of the packed kernel), a CTA prefix sum over the lengths, the strings
+ *                 concatenated into the chunk's word-aligned string in its area of the segment's slot; the chunk's bit
+ *                 offset in the segment by a decoupled look-back over the chunks in front of it (64-bit: a scan of a 2^30-pixel
+ *                 frame can exceed 2^32 bits).  The DC predictor is read from the coefficient buffer, so it crosses chunks.
+ *   k_huff_stuff  one CTA per tile of GJ_HS_TILE bytes of a segment's unstuffed image, gathered from the chunk strings by funnel
+ *                 shifts (gj_hs_gather) and padded at the segment's end; the tile counts its 0xFF bytes, finds its stream
+ *                 offset by a decoupled look-back over the tiles in stream order (what precedes a scan, RSTn and EOI
+ *                 included) and writes its stuffed bytes straight into the stream.
+ * Status words of both look-backs: HS_AGG | the item's own sum, then HS_INC | the sum up to and including it. */
+#define HS_AGG (1ull << 62)
+#define HS_INC (1ull << 63)
+#define HS_VALUE (HS_AGG - 1ull)
+constexpr int HC_PRIV = 55;   // words per thread: a block never needs more than 54 (odd stride: conflict-free columns)
+constexpr int HC_SMEM = (2 * 256 + 2 * 16 + GJ_HS_CHUNK * HC_PRIV + 4 + GJ_HS_CHUNK * HE_HEAD + 32) * 4;
+constexpr int HT_THREADS = 256;
+constexpr int HT_WPT = GJ_HS_TILE / 4 / HT_THREADS;          // image words per thread
+constexpr int HT_MAXCH = GJ_HS_TILE * 8 / (2 * GJ_HS_CHUNK) + 2;   // chunks a tile can touch (a block is >= 2 bits)
+
+/* sum of the status values from item j backwards to the first inclusive one; prev(j): the item in front of j, or -1 */
+template <class Prev>
+__device__ __forceinline__ uint64_t hs_look_back(volatile unsigned long long* status, long long j, Prev prev)
+{
+    uint64_t sum = 0;
+    while ( j >= 0 ) {
+        unsigned long long v;
+        do {
+            v = status[j];
+        } while ( v == 0ull );
+        sum += v & HS_VALUE;
+        if ( v & HS_INC ) break;
+        j = prev(j);
+    }
+    return sum;
+}
+
+__device__ __forceinline__ int hs_cta_excl_scan(int v, int& total, int* s_warp)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    const int incl = warp_incl_scan(v, lane);
+    if ( lane == 31 ) s_warp[warp] = incl;
+    __syncthreads();
+    int before = 0;
+    total = 0;
+    for ( int w = 0; w < nwarps; w++ ) {
+        const int t = s_warp[w];
+        if ( w < warp ) before += t;
+        total += t;
+    }
+    return before + incl - v;
+}
+
+/* blocks of segment g, its scan and number in the scan */
+__device__ __forceinline__ int hs_segment(const gj_scan_layout& L, int seg_mcu, int g, int& scan, int& s)
+{
+    scan = scan_of_segment(L, g);
+    s = g - L.scan_seg_begin[scan];
+    return min(seg_mcu, L.scan_mcus[scan] - s * seg_mcu) * L.bpm;
+}
+
+__global__ void __launch_bounds__(GJ_HS_CHUNK)
+k_huff_chunk(const int16_t* __restrict__ coef, const uint64_t* __restrict__ nzmask, const __grid_constant__ gj_scan_layout lay,
+             int seg_mcu, int nch, uint8_t* __restrict__ tmp, size_t slot_stride, const gj_dev_enc_tables* __restrict__ tables,
+             uint64_t* __restrict__ info, volatile unsigned long long* chunk_status)
+{
+    gj_pdl_wait();
+    extern __shared__ __align__(16) uint32_t hc_smem[];
+    uint32_t (*s_ac)[256] = reinterpret_cast<uint32_t (*)[256]>(hc_smem);
+    uint32_t (*s_dc)[16] = reinterpret_cast<uint32_t (*)[16]>(hc_smem + 512);
+    uint32_t* s_priv = hc_smem + 512 + 32;
+    uint32_t* s_head = s_priv + GJ_HS_CHUNK * HC_PRIV + 4;   // 16-byte aligned
+    int* s_warp = reinterpret_cast<int*>(s_head + GJ_HS_CHUNK * HE_HEAD);
+
+    const int g = blockIdx.x / nch, c = blockIdx.x - g * nch;
+    int scan, s;
+    const int nblocks = hs_segment(lay, seg_mcu, g, scan, s);
+    const int j0 = c * GJ_HS_CHUNK;
+    if ( j0 >= nblocks ) return;   // the last segment of a scan may have fewer chunks
+    for ( int i = threadIdx.x; i < 512; i += blockDim.x )
+        s_ac[i >> 8][i & 255] = tables->lut[i >> 8].ac[i & 255];
+    if ( threadIdx.x < 32 ) s_dc[threadIdx.x >> 4][threadIdx.x & 15] = tables->lut[threadIdx.x >> 4].dc[threadIdx.x & 15];
+    __syncthreads();
+
+    const int first_mcu = s * seg_mcu, j = j0 + (int)threadIdx.x;
+    uint32_t* priv = s_priv + threadIdx.x * HC_PRIV;
+    int len = 0;
+    if ( j < nblocks ) {
+        size_t bi;
+        int comp, pd;
+        segment_block(lay, scan, first_mcu, j, bi, comp, pd);
+        uint32_t* head = s_head + threadIdx.x * HE_HEAD;
+        const int16_t* blk = coef + bi * 64;
+        const uint64_t nz = __ldg(nzmask + bi);
+        const uint4 ha = __ldg(reinterpret_cast<const uint4*>(blk)), hb = __ldg(reinterpret_cast<const uint4*>(blk) + 1);
+        /* DC predictor: previous block of the same component inside the segment, 0 at its start -- in this chunk or not */
+        int pred = 0;
+        if ( j >= pd ) {
+            size_t bp;
+            int cp, pp;
+            segment_block(lay, scan, first_mcu, j - pd, bp, cp, pp);
+            pred = __ldg(coef + bp * 64);
+        }
+        reinterpret_cast<uint4*>(head)[0] = ha;   // only this thread reads its head
+        reinterpret_cast<uint4*>(head)[1] = hb;
+        len = code_block((int)(short)(ha.x & 0xFFFFu), pred, nz, reinterpret_cast<const int16_t*>(head), blk, s_ac, s_dc,
+                         lay.comp_tbl[comp], [&](int wi, uint32_t w) { priv[wi] = w; });
+    }
+    int total;
+    const int excl = hs_cta_excl_scan(len, total, s_warp);
+
+    /* the chunk's offset in its segment */
+    const long long me = blockIdx.x;
+    if ( threadIdx.x == 0 ) {
+        unsigned long long before = 0;
+        if ( c == 0 ) chunk_status[me] = HS_INC | (unsigned long long)total;
+        else {
+            chunk_status[me] = HS_AGG | (unsigned long long)total;
+            before = hs_look_back(chunk_status, me - 1, [&](long long q) { return q - 1 > (long long)g * nch - 1 ? q - 1 : -1ll; });
+            chunk_status[me] = HS_INC | (before + (unsigned long long)total);
+        }
+    }
+
+    /* the chunk's area in the segment's slot: its share of the slot's words per block */
+    const int segblk = seg_mcu * lay.bpm;
+    const uint32_t share = (uint32_t)(slot_stride / 4 / (size_t)segblk);
+    const int nblk = min(GJ_HS_CHUNK, nblocks - j0);
+    const uint32_t nw = ((uint32_t)total + 31u) >> 5;
+    if ( nw > (uint32_t)nblk * share ) {   // the slot is too small: the size it needs -> info[2], the host encodes again
+        if ( threadIdx.x == 0 ) {
+            atomicOr(reinterpret_cast<unsigned long long*>(info + 1), 2ull);
+            const unsigned long long need = (unsigned long long)((nw + nblk - 1) / nblk) * 4ull * (unsigned long long)segblk;
+            atomicMax(reinterpret_cast<unsigned long long*>(info + 2), need);
+        }
+        return;
+    }
+    uint32_t* area = reinterpret_cast<uint32_t*>(tmp + (size_t)g * slot_stride) + (size_t)j0 * share;
+    /* words shared with a neighbouring block are cleared first, then ORed into; words inside one block are plain stores */
+    if ( len ) {
+        area[excl >> 5] = 0u;
+        area[(excl + len - 1) >> 5] = 0u;
+    }
+    __syncthreads();
+    if ( len ) {
+        const int nwb = (len + 31) >> 5;
+        const int d0 = excl >> 5, sh = excl & 31, endbit = excl + len;
+        uint32_t prev = 0;
+        for ( int q = 0; q <= nwb; q++ ) {
+            const uint32_t w = q < nwb ? priv[q] : 0u;
+            const uint32_t o = sh ? (prev | (w >> sh)) : w;
+            prev = sh ? (w << (32 - sh)) : 0u;
+            const int d = d0 + q;
+            if ( 32 * d >= endbit ) break;
+            if ( 32 * d >= excl && 32 * d + 32 <= endbit ) area[d] = o;
+            else atomicOr(&area[d], o);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(HT_THREADS)
+k_huff_stuff(const uint8_t* __restrict__ tmp, size_t slot_stride, const __grid_constant__ gj_scan_layout lay, int seg_mcu, int nch,
+             int tps, const unsigned long long* __restrict__ chunk_status, const uint8_t* __restrict__ sos,
+             const __grid_constant__ ScanPrefix pre, uint32_t header_size, uint64_t stream_cap, uint8_t* __restrict__ stream,
+             volatile unsigned long long* tile_status, uint64_t* __restrict__ seg_pos, uint64_t* __restrict__ info,
+             uint64_t* __restrict__ info_next)
+{
+    gj_pdl_wait();
+    __shared__ __align__(16) uint8_t s_out[2 * GJ_HS_TILE];
+    __shared__ unsigned long long s_end[HT_MAXCH];
+    __shared__ int s_warp[HT_THREADS / 32];
+    __shared__ unsigned long long s_base;
+    const int seg_count = lay.scan_seg_begin[GJ_MAX_COMP];
+    if ( info[1] & 2ull ) {   // a slot was too small (k_huff_chunk): the host encodes again
+        if ( blockIdx.x == 0 && threadIdx.x == 0 && info_next ) info_next[0] = info_next[1] = info_next[2] = info_next[3] = 0ull;
+        return;
+    }
+    const int g = (int)(blockIdx.x / (unsigned)tps);
+    const long long i = (long long)blockIdx.x - (long long)g * tps;
+    int scan, s;
+    const int nblocks = hs_segment(lay, seg_mcu, g, scan, s);
+    const int nch_g = gj_hs_chunks(nblocks);
+    const unsigned long long* E = chunk_status + (size_t)g * nch;
+    const uint64_t bits = E[nch_g - 1] & HS_VALUE;
+    const long long ntiles = (long long)gj_hs_tiles(bits);
+    if ( i >= ntiles ) return;
+    const uint64_t nbytes = gj_hs_seg_bytes(bits);
+    const uint64_t P0 = (uint64_t)i * GJ_HS_TILE * 8;
+    const uint32_t tile_bytes = (uint32_t)min((uint64_t)GJ_HS_TILE, nbytes - (uint64_t)i * GJ_HS_TILE);
+
+    /* the first chunk that ends behind the tile's first bit: a 256-ary search over the chunk ends */
+    int lo = 0, hi = nch_g - 1;   // E[hi] = bits > P0
+    while ( lo < hi ) {
+        const int step = (hi - lo + HT_THREADS - 1) / HT_THREADS;
+        const int c = lo + (int)threadIdx.x * step;
+        const int cnt = __syncthreads_count(c < hi && (E[c] & HS_VALUE) <= P0);
+        const int nlo = cnt ? lo + (cnt - 1) * step + 1 : lo;
+        hi = min(hi, lo + cnt * step);
+        lo = nlo;
+    }
+    const int c0 = lo;
+    const int kn = min(HT_MAXCH, nch_g - c0);
+    for ( int k = threadIdx.x; k < kn; k += HT_THREADS )
+        s_end[k] = E[c0 + k] & HS_VALUE;
+    const uint64_t o0 = c0 ? (E[c0 - 1] & HS_VALUE) : 0ull;
+    __syncthreads();
+
+    /* this thread's HT_WPT words of the image, gathered from the chunks (chunk c at its area: c * GJ_HS_CHUNK shares) */
+    const uint32_t share = (uint32_t)(slot_stride / 4 / (size_t)(seg_mcu * lay.bpm));
+    const uint32_t* slot = reinterpret_cast<const uint32_t*>(tmp + (size_t)g * slot_stride);
+    const uint32_t b0 = threadIdx.x * HT_WPT * 4;
+    const uint32_t my_bytes = tile_bytes > b0 ? min(tile_bytes - b0, (uint32_t)HT_WPT * 4) : 0u;
+    uint32_t w[HT_WPT];
+    int cnt = (int)my_bytes;
+    int k = 0;
+#pragma unroll
+    for ( int r = 0; r < HT_WPT; r++ ) {
+        w[r] = 0u;
+        if ( 4u * r >= my_bytes ) continue;
+        const uint64_t p = P0 + 8ull * (b0 + 4u * r);
+        if ( p < bits ) {
+            while ( k + 1 < kn && s_end[k] <= p ) k++;
+            const uint64_t o = k ? s_end[k - 1] : o0, e = s_end[k];
+            const int c = c0 + k;
+            const uint32_t next0 = e - p < 32 && c + 1 < nch_g ? slot[(size_t)(c + 1) * GJ_HS_CHUNK * share] : 0u;
+            w[r] = gj_hs_gather(slot + (size_t)c * GJ_HS_CHUNK * share, o, e, next0, p);
+        }
+        w[r] = gj_hs_pad(w[r], p, bits);
+        cnt += gj_hs_ff_count(w[r] & gj_hs_keep(my_bytes - 4u * r));
+    }
+    int stuffed;
+    const int at = hs_cta_excl_scan(cnt, stuffed, s_warp);
+    {
+        uint8_t* o = s_out + at;
+#pragma unroll
+        for ( int r = 0; r < HT_WPT; r++ )
+#pragma unroll
+            for ( int x = 0; x < 4; x++ )
+                if ( 4u * r + x < my_bytes ) {
+                    const uint8_t b = (uint8_t)(w[r] >> (24 - 8 * x));
+                    *o++ = b;
+                    if ( b == 0xFF ) *o++ = 0;
+                }
+    }
+
+    /* stream offset: everything in front of this tile, in stream order */
+    const int segs = lay.scan_seg_begin[scan + 1] - lay.scan_seg_begin[scan];
+    const bool last_tile = i + 1 == ntiles, last_seg = g + 1 == seg_count;
+    const uint32_t front = i == 0 ? gj_hs_seg_front(s, (uint32_t)pre.len[scan]) : 0u;
+    const uint32_t back = last_tile ? gj_hs_seg_back(s, segs, last_seg) : 0u;
+    const unsigned long long mine = front + (unsigned long long)stuffed + back;
+    if ( threadIdx.x == 0 ) {
+        const long long me = blockIdx.x;
+        unsigned long long before = 0;
+        if ( me == 0 ) tile_status[me] = HS_INC | mine;
+        else {
+            tile_status[me] = HS_AGG | mine;
+            /* the tile in front: the previous tile of the segment, or the last tile of the previous segment */
+            auto prev = [&](long long q) -> long long {
+                const int gq = (int)(q / tps);
+                if ( q - (long long)gq * tps > 0 ) return q - 1;
+                if ( gq == 0 ) return -1;
+                int sc, ss;
+                const int nb = hs_segment(lay, seg_mcu, gq - 1, sc, ss);
+                const uint64_t b = chunk_status[(size_t)(gq - 1) * nch + gj_hs_chunks(nb) - 1] & HS_VALUE;
+                return (long long)(gq - 1) * tps + (long long)gj_hs_tiles(b) - 1;
+            };
+            before = hs_look_back(tile_status, prev(me), prev);
+            tile_status[me] = HS_INC | (before + mine);
+        }
+        s_base = header_size + before;
+        if ( last_seg && last_tile ) {
+            const uint64_t end = header_size + before + mine;
+            info[0] = end;
+            info[1] = end > stream_cap ? 1ull : 0ull;
+            if ( info_next ) info_next[0] = info_next[1] = info_next[2] = info_next[3] = 0ull;
+        }
+    }
+    __syncthreads();
+    const uint64_t base = s_base;
+    if ( base + mine > stream_cap ) return;   // the host reports the error (info[1] bit 0)
+    if ( front ) {
+        const uint8_t* from = sos + pre.off[scan];
+        for ( uint32_t q = threadIdx.x; q < front; q += HT_THREADS )
+            stream[base + q] = from[q];
+    }
+    const uint64_t off = base + front;
+    if ( i == 0 && seg_pos && threadIdx.x == 0 ) seg_pos[g] = off;
+    /* the stuffed bytes: up to 16-byte alignment of the destination, then 16-byte stores */
+    uint8_t* dst = stream + off;
+    const uint32_t n = (uint32_t)stuffed;
+    const uint32_t head = min(n, (uint32_t)((16 - (reinterpret_cast<uintptr_t>(dst) & 15)) & 15));
+    for ( uint32_t q = threadIdx.x; q < head; q += HT_THREADS )
+        dst[q] = s_out[q];
+    const uint32_t nvec = (n - head) >> 4;
+    for ( uint32_t q = threadIdx.x; q < nvec; q += HT_THREADS ) {
+        const uint8_t* f = s_out + head + 16 * q;
+        uint32_t v[4];
+#pragma unroll
+        for ( int x = 0; x < 4; x++ )
+            v[x] = (uint32_t)f[4 * x] | (uint32_t)f[4 * x + 1] << 8 | (uint32_t)f[4 * x + 2] << 16 | (uint32_t)f[4 * x + 3] << 24;
+        reinterpret_cast<uint4*>(dst + head)[q] = make_uint4(v[0], v[1], v[2], v[3]);
+    }
+    for ( uint32_t q = head + (nvec << 4) + threadIdx.x; q < n; q += HT_THREADS )
+        dst[q] = s_out[q];
+    if ( back && threadIdx.x == 0 ) {
+        /* RSTn, n = index in scan mod 8 [ref: src/gpujpeg_huffman_cpu_encoder.c:366-367], or EOI */
+        dst[n] = 0xFF;
+        dst[n + 1] = s + 1 < segs ? (uint8_t)(0xD0 + (s & 7)) : (uint8_t)0xD9;
     }
 }
 
@@ -1333,6 +1614,53 @@ extern "C" int gj_launch_huffman_place(const struct gj_huff_enc_args* a, gj_stre
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
+/* status words of the long-segment path: one per chunk, then one per tile of slots of at most max_slot_stride bytes */
+extern "C" size_t gj_huffman_split_status_bytes(int seg_count, int segblk, size_t max_slot_stride)
+{
+    if ( segblk <= HP_MAXBLK ) return 0;
+    return (size_t)gj_hs_status_words(seg_count, segblk, max_slot_stride) * sizeof(uint64_t);
+}
+
+/* segments longer than HP_MAXBLK blocks: k_huff_chunk, then k_huff_stuff over as many tiles per segment as its slot can
+ * hold (the tiles behind a segment's end return at once) */
+static int launch_split(const struct gj_huff_enc_args* a, gj_stream_t stream)
+{
+    const int seg_count = a->lay.scan_seg_begin[GJ_MAX_COMP];
+    const int nch = gj_hs_chunks(a->seg_mcu * a->lay.bpm);
+    const uint64_t tps = gj_hs_tiles_per_slot(a->slot_stride);
+    const size_t chunks = (size_t)seg_count * nch, tiles = (size_t)seg_count * tps;
+    if ( gj_hs_status_words(seg_count, a->seg_mcu * a->lay.bpm, a->slot_stride) * sizeof(uint64_t) > a->split_bytes ||
+         chunks > 0x7FFFFFFFu || tiles > 0x7FFFFFFFu )
+        return -1;
+    if ( !a->info_is_zero && cudaMemsetAsync(a->d_info, 0, 32, stream) != cudaSuccess ) return -1;
+    if ( cudaMemsetAsync(a->d_split, 0, (chunks + tiles) * sizeof(uint64_t), stream) != cudaSuccess ) return -1;
+    unsigned long long* chunk_status = reinterpret_cast<unsigned long long*>(a->d_split);
+    ScanPrefix pre;
+    for ( int k = 0; k < GJ_MAX_COMP; k++ ) {
+        pre.len[k] = a->pre_len[k];
+        pre.off[k] = a->pre_off[k];
+    }
+    gj_launch_pdl(k_huff_chunk, dim3((unsigned)chunks), dim3(GJ_HS_CHUNK), HC_SMEM, stream, a->d_coef, a->d_nzmask, a->lay, a->seg_mcu,
+                  nch, a->d_tmp, a->slot_stride, a->d_tables, a->d_info, (volatile unsigned long long*)chunk_status);
+    gj_launch_pdl(k_huff_stuff, dim3((unsigned)tiles), dim3(HT_THREADS), 0, stream, (const uint8_t*)a->d_tmp, a->slot_stride, a->lay,
+                  a->seg_mcu, nch, (int)tps, (const unsigned long long*)chunk_status, a->d_sos, pre, a->header_size,
+                  (uint64_t)a->stream_cap, a->d_stream, (volatile unsigned long long*)(chunk_status + chunks), a->d_seg_pos, a->d_info,
+                  a->d_info_next);
+    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+/* Segments longer than HP_MAXBLK blocks: one warp per segment (k_huff_encode) for segments of a few hundred blocks when they
+ * fill the machine, chunks of blocks (launch_split) otherwise.  K2 in us, k_huff_encode / chunks, of photo q75 frames by
+ * blocks per segment and segments (profiles/nodri_encode.py, H100 80GB HBM3 at a 700 W power limit):
+ *   41-42 blocks   8K 4:4:4 37 932 segments 155 / 960, 8K 4:2:0 18 514: 121 / 543, HD 4:4:4 2 371: 30 / 85, HD 4:2:0 1 157: 28 / 59
+ *   100 blocks     8K 15 552: 135 / 440, 4K 3 888: 58 / 129, HD 972: 38 / 49
+ *   300 blocks     4K 1 296: 87 / 102, HD 324: 68 / 51
+ *   600 blocks     8K 1 296: 176 / 157, 4K 324: 138 / 60, HD 81: 135 / 37
+ *   1000+ blocks   8K 4:4:4 1 555: 284 / 207, HD 98: 215 / 40; restart_interval = 0 (8K): 116 801 / 250 */
+constexpr int HE_WARP_MAXBLK = 512;     // longer segments always take the chunks
+constexpr int HE_WARP_SHORT = 256;      // shorter ones always take a warp each
+constexpr int HE_WARP_SEGS_PER_SM = 8;  // in between: a warp each when there are at least this many segments per SM
+
 extern "C" int gj_launch_huffman_encode(const struct gj_huff_enc_args* a, gj_stream_t stream)
 {
     const int seg_count = a->lay.scan_seg_begin[GJ_MAX_COMP];
@@ -1341,6 +1669,10 @@ extern "C" int gj_launch_huffman_encode(const struct gj_huff_enc_args* a, gj_str
         for ( int k = 0; k < a->lay.scan_count && k < GJ_MAX_COMP; k++ )
             n[k] = a->lay.scan_seg_begin[k + 1] - a->lay.scan_seg_begin[k];
         if ( gj_launch_huffman_encode_part(a, 1, lo, n, stream) ) return -1;
+    }
+    else if ( a->seg_mcu * a->lay.bpm >= HE_WARP_MAXBLK ||
+              (a->seg_mcu * a->lay.bpm >= HE_WARP_SHORT && seg_count < HE_WARP_SEGS_PER_SM * gj_cuda_sm_count()) ) {
+        return launch_split(a, stream);
     }
     else {
         if ( !a->info_is_zero && cudaMemsetAsync(a->d_info, 0, 32, stream) != cudaSuccess ) return -1;

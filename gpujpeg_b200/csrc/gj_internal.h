@@ -424,8 +424,12 @@ struct gj_huff_enc_args {
     uint64_t* d_info_next;  /* [4] or NULL: cleared by this launch for the next one */
     int info_is_zero;       /* d_info has been cleared by the previous launch */
     const struct gj_dev_enc_tables* d_tables;
+    uint64_t* d_split;      /* segments longer than 40 blocks: status words of the chunks and tiles, split_bytes bytes */
+    size_t split_bytes;
 };
 int gj_launch_huffman_encode(const struct gj_huff_enc_args* a, gj_stream_t stream);
+/* bytes of d_split a frame needs whose slots grow to at most max_slot_stride bytes (0: short segments) */
+size_t gj_huffman_split_status_bytes(int seg_count, int segblk, size_t max_slot_stride);
 /* the same in pieces (the encoder's stripe pipeline): K2 on scan k's segments [lo[k], lo[k] + n[k]) -- `first` marks the first
  * piece of a frame --, then the tail kernel once; only for frames gj_huffman_encode_parts_eligible() accepts */
 int gj_huffman_encode_parts_eligible(const struct gj_huff_enc_args* a);
