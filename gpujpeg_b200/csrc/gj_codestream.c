@@ -514,6 +514,76 @@ int gj_k3_choose(const struct gj_geometry* g, int request, const int force_lanes
     return pick;
 }
 
+/* - The fused kernels write RGB as they transform, at full size only, and flip only a frame without vertical padding: flipping
+ *   the padded planes and then replicating chrominance rows is flipping the finished image only then [ref:
+ *   src/gpujpeg_postprocessor.cu:447], and the fused kernels do that by writing the rows last to first.  Any other RGB frame
+ *   takes the planes and the generic pass.
+ * - The sample kernels write blocks where they stand: a turned or mirrored frame takes the planes and the generic pass.
+ * - dec_opt_pixels=libjpeg: the ISLOW instance of k_idct_samples on the raw coefficients into the planes, of a cropped frame
+ *   the blocks of its rectangle widened for the upsampling's neighbours (gj_crop_widen), then the pass that upsamples,
+ *   converts, orients and crops.  A grey frame as stored has nothing to upsample or convert: it goes straight to the output.
+ * - The reduced IDCTs, ISLOW and the float flavour read raw coefficients; the integer IDCT has K3 dequantise. */
+void gj_k4_choose(const struct gj_geometry* g, const struct gj_k4_request* r, struct gj_k4_plan* p)
+{
+    memset(p, 0, sizeof *p);
+    int out = r->out;
+    if ( r->scale > 1 && out == GJ_OUT_RGB ) out = GJ_OUT_GENERIC;
+    if ( r->orient && out == GJ_OUT_SAMPLES ) out = GJ_OUT_GENERIC;
+    if ( r->flipped && !(out == GJ_OUT_RGB && g->height % (8 * g->max_vs) == 0) ) out = GJ_OUT_GENERIC;
+    p->flavour = r->libjpeg ? GJ_IDCT_ISLOW : r->idct_flavour;
+    p->dequantize = r->idct_flavour == 0 && r->scale == 1 && !r->coef_only && !r->libjpeg;
+    p->n = 8 / r->scale;
+    p->map = r->map;
+    p->mcu_rows = (g->bcy + g->max_vs - 1) / g->max_vs;
+    if ( r->crop ) {
+        int w[4] = {r->src[0], r->src[1], r->src[2], r->src[3]};
+        if ( r->libjpeg ) gj_crop_widen(g->width, g->height, g->max_hs, g->max_vs, w);
+        gj_crop_blocks(g, p->n, w[0], w[1], w[2], w[3], p->win.blk);
+    }
+    if ( r->libjpeg ) {
+        p->kernel = GJ_K4_SAMPLES;
+        p->window = r->crop;
+        if ( g->comp_count == 1 && !r->orient ) {
+            p->scomp = 1;
+            if ( r->crop ) {
+                p->win.ox[0] = r->src[0];
+                p->win.oy[0] = r->src[1];
+            }
+        }
+        else {
+            p->to_planes = 1;
+            p->post = GJ_K4_POST_LIBJPEG;
+            p->post_map = 1;
+        }
+    }
+    else if ( out == GJ_OUT_RGB ) {
+        p->kernel = GJ_K4_FUSED;
+        p->window = r->crop || r->orient;
+        memcpy(p->rect, r->src, sizeof p->rect);
+        p->orient = !r->orient ? 0 : r->map.sxx == 0 ? 2 : 1;
+        p->flip = r->flipped && !p->window ? GJ_K4_FLIP_PITCH : GJ_K4_FLIP_NONE;
+        p->stripes = !r->flipped && !r->channel_remap && !p->window && !r->coef_only;
+    }
+    else {
+        p->kernel = r->scale > 1 ? GJ_K4_SCALED : GJ_K4_SAMPLES;
+        p->window = r->crop;
+        if ( out == GJ_OUT_SAMPLES ) {
+            p->scomp = r->scale > 1 || r->crop;
+            for ( int c = 0; c < g->comp_count && r->crop; c++ ) {
+                p->win.ox[c] = r->src[0] / (g->max_hs / g->comp[c].hs);
+                p->win.oy[c] = r->src[1] / (g->max_vs / g->comp[c].vs);
+            }
+        }
+        else {
+            p->to_planes = 1;
+            p->flip = r->flipped && !r->crop && r->scale == 1 ? GJ_K4_FLIP_PLANES : GJ_K4_FLIP_NONE;
+            p->post = GJ_K4_POST_CONVERT;
+            p->post_map = r->crop || r->orient;
+        }
+    }
+    p->planes_bytes = p->to_planes ? g->coef_count / 64 * (size_t)(p->n * p->n) : 0;
+}
+
 /* ------------------------------------------------------------------------------------------- */
 /* writer                                                                                        */
 

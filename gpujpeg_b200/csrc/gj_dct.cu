@@ -28,6 +28,9 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <tuple>
+#include <type_traits>
+
 #include "gj_device.cuh"
 #include "gj_internal.h"
 #include "gj_launch.cuh"
@@ -1404,6 +1407,34 @@ int pick_vec(const void* p, size_t pitch)
     return (a & 3) == 0 ? 4 : 1;
 }
 
+/* K4's template instances from runtime values: OneOf<candidates...>{value} for every template argument, and a generic lambda
+ * that takes one std::integral_constant per argument; -1 if a value is none of its candidates */
+template <auto... Vs>
+struct OneOf {
+    int v;
+};
+template <class F, class... Cs>
+int instance(F& f, std::tuple<Cs...>)
+{
+    return f(Cs{}...);
+}
+template <class F, class... Cs, auto... Vs, class... Rest>
+int instance(F& f, std::tuple<Cs...>, OneOf<Vs...> x, Rest... rest)
+{
+    int rc = -1;
+    (void)((x.v == (int)Vs && (rc = instance(f, std::tuple<Cs..., std::integral_constant<decltype(Vs), Vs>>{}, rest...), true)) || ...);
+    return rc;
+}
+
+/* the dequantisation tables of the frame's components */
+IdctParams idct_params(const struct gj_dev_dec_tables* h_tables, const int* comp_tq, int comp_count)
+{
+    IdctParams prm;
+    for ( int c = 0; c < GJ_MAX_COMP; c++ )
+        memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c < comp_count ? c : 0]], sizeof prm.q_zz[c]);
+    return prm;
+}
+
 }  // namespace
 
 /* `bcy` block rows starting at the pointers given; `nblk` = blocks of a whole component plane (the distance between the
@@ -1468,48 +1499,6 @@ extern "C" int gj_launch_fdct_rgb444_rows(const uint8_t* d_raw, int width, int h
     const int rows = (by1 * 8 < height ? by1 * 8 : height) - by0 * 8;
     return launch_fdct_rgb444(d_raw + (ptrdiff_t)by0 * 8 * pitch, width, rows, pitch, d_coef + (size_t)by0 * bcx * 64,
                               d_nzmask + (size_t)by0 * bcx, bcx, by1 - by0, bcx * bcy, h_tables, stream);
-}
-
-static int launch_idct_rgb444(const int16_t* d_coef, const uint8_t* d_cext, int bcx, int bcy, int nblk, const int comp_tq[3],
-                              uint8_t* d_raw, int width, int height, int pitch, int idct_flavour, int coef_dequantized,
-                              const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
-{
-    IdctParams prm;
-    for ( int c = 0; c < 3; c++ )
-        memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c]], sizeof prm.q_zz[c]);
-    const dim3 grid((bcx + TB - 1) / TB, bcy);
-    const int vec = pick_vec(d_raw, (size_t)pitch);
-    if ( idct_flavour != 0 && coef_dequantized ) return -1;   // the float flavour needs raw coefficients
-    const FusedWin nowin = {};
-#define GJ_K4(V, F, D) gj_launch_pdl(k_idct_rgb444<V, F, D, false>, grid, dim3(NT), 0, stream, d_coef, d_cext, bcx, nblk, d_raw, width, height, (size_t)pitch, prm, nowin)
-    if ( idct_flavour == 0 && coef_dequantized ) {
-        if ( vec == 4 ) GJ_K4(4, 0, false); else GJ_K4(1, 0, false);
-    }
-    else if ( idct_flavour == 0 ) {
-        if ( vec == 4 ) GJ_K4(4, 0, true); else GJ_K4(1, 0, true);
-    }
-    else {
-        if ( vec == 4 ) GJ_K4(4, 1, true); else GJ_K4(1, 1, true);
-    }
-#undef GJ_K4
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
-}
-extern "C" int gj_launch_idct_rgb444(const int16_t* d_coef, const uint8_t* d_cext, int bcx, int bcy, const int comp_tq[3],
-                                     uint8_t* d_raw, int width, int height, int pitch, int idct_flavour, int coef_dequantized,
-                                     const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
-{
-    return launch_idct_rgb444(d_coef, d_cext, bcx, bcy, bcx * bcy, comp_tq, d_raw, width, height, pitch, idct_flavour, coef_dequantized,
-                              h_tables, stream);
-}
-/* block rows [by0, by1) only (the decoder's stripe pipeline: finished rows leave for the host while later rows are transformed) */
-extern "C" int gj_launch_idct_rgb444_rows(const int16_t* d_coef, const uint8_t* d_cext, int bcx, int bcy, int by0, int by1,
-                                          const int comp_tq[3], uint8_t* d_raw, int width, int height, int pitch, int idct_flavour,
-                                          int coef_dequantized, const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
-{
-    if ( by0 < 0 || by1 > bcy || by0 >= by1 ) return -1;
-    const int rows = (by1 * 8 < height ? by1 * 8 : height) - by0 * 8;
-    return launch_idct_rgb444(d_coef + (size_t)by0 * bcx * 64, d_cext + (size_t)by0 * bcx, bcx, by1 - by0, bcx * bcy, comp_tq, d_raw + (ptrdiff_t)by0 * 8 * pitch,
-                              width, rows, pitch, idct_flavour, coef_dequantized, h_tables, stream);
 }
 
 /* ---- subsampled variants: luminance hs x vs in {2x1, 2x2, 1x2}, chrominance 1x1 ---- */
@@ -1639,134 +1628,6 @@ extern "C" int gj_launch_fdct_libjpeg(const uint8_t* d_raw, int width, int heigh
                                        raw_q, stream);
 }
 
-extern "C" int gj_launch_idct_rgb_ss_rows(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], int my0, int my1,
-                                          const int comp_tq[3], uint8_t* d_raw, int width, int height, int pitch, int idct_flavour,
-                                          int coef_dequantized, const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
-{
-    IdctParams prm;
-    for ( int c = 0; c < 3; c++ )
-        memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c]], sizeof prm.q_zz[c]);
-    const int hs = comp[0].hs, vs = comp[0].vs;
-    if ( comp[1].hs != 1 || comp[1].vs != 1 || comp[2].hs != 1 || comp[2].vs != 1 ) return -1;
-    if ( idct_flavour != 0 && coef_dequantized ) return -1;
-    const int mcu_rows = (comp[0].bcy + vs - 1) / vs;
-    if ( my0 < 0 || my1 > mcu_rows || my0 >= my1 ) return -1;
-    SsGrid sg;
-    height = ss_grid_rows(&sg, comp, my0, my1, height);
-    d_raw += (ptrdiff_t)my0 * 8 * vs * pitch;
-    const dim3 grid((comp[0].bcx + TB - 1) / TB, my1 - my0);
-    const int vec = pick_vec(d_raw, (size_t)pitch);
-    const FusedWin nowin = {};
-#define GJ_K4SS2(H, V, VE, F, D) \
-    gj_launch_pdl(k_idct_rgb_ss<H, V, VE, F, D, false>, grid, dim3(TB * V + 2 * TB / H), 0, stream, d_coef, d_cext, sg, d_raw, width, height, (size_t)pitch, prm, nowin)
-#define GJ_K4SS(H, V)                                                                  \
-    do {                                                                               \
-        if ( idct_flavour == 0 && coef_dequantized ) {                                 \
-            if ( vec == 4 ) GJ_K4SS2(H, V, 4, 0, false); else GJ_K4SS2(H, V, 1, 0, false); \
-        }                                                                              \
-        else if ( idct_flavour == 0 ) {                                                \
-            if ( vec == 4 ) GJ_K4SS2(H, V, 4, 0, true); else GJ_K4SS2(H, V, 1, 0, true);   \
-        }                                                                              \
-        else {                                                                         \
-            if ( vec == 4 ) GJ_K4SS2(H, V, 4, 1, true); else GJ_K4SS2(H, V, 1, 1, true);   \
-        }                                                                              \
-    } while ( 0 )
-    if ( hs == 2 && vs == 2 ) GJ_K4SS(2, 2);
-    else if ( hs == 2 && vs == 1 ) GJ_K4SS(2, 1);
-    else if ( hs == 1 && vs == 2 ) GJ_K4SS(1, 2);
-    else return -1;
-#undef GJ_K4SS
-#undef GJ_K4SS2
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
-}
-extern "C" int gj_launch_idct_rgb_ss(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], const int comp_tq[3],
-                                     uint8_t* d_raw, int width, int height, int pitch, int idct_flavour,
-                                     int coef_dequantized, const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
-{
-    const int vs = comp[0].vs > 0 ? comp[0].vs : 1;
-    return gj_launch_idct_rgb_ss_rows(d_coef, d_cext, comp, 0, (comp[0].bcy + vs - 1) / vs, comp_tq, d_raw, width, height, pitch,
-                                      idct_flavour, coef_dequantized, h_tables, stream);
-}
-
-/* dec_opt_crop on the fused kernels: the rectangle [x, x + w) x [y, y + h) of the RGB image into d_out (pitch 3w); 4:4:4 when
- * every component is 1x1, else the chroma-subsampling instance.  dec_opt_orientation: the ORIENT instances, `orient` mapping the
- * rectangle to the output (h x w pixels, pitch 3h, for a quarter turn). */
-extern "C" int gj_launch_idct_rgb_window(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3], const int comp_tq[3],
-                                         uint8_t* d_out, int width, int height, int x, int y, int w, int h, int idct_flavour,
-                                         int coef_dequantized, const struct gj_orient_map* orient, const struct gj_dev_dec_tables* h_tables,
-                                         gj_stream_t stream)
-{
-    IdctParams prm;
-    for ( int c = 0; c < 3; c++ )
-        memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c]], sizeof prm.q_zz[c]);
-    if ( idct_flavour != 0 && coef_dequantized ) return -1;
-    if ( w < 1 || h < 1 || x < 0 || y < 0 || x + w > width || y + h > height ) return -1;
-    const int hs = comp[0].hs, vs = comp[0].vs;
-    if ( comp[1].hs != 1 || comp[1].vs != 1 || comp[2].hs != 1 || comp[2].vs != 1 ) return -1;
-    const int quarter = orient && orient->sxx == 0;
-    /* the pixels a CTA covers: a 512-pixel strip of an MCU row, or a quarter turn's 64 x 64 * vs tile */
-    const int tw = quarter ? QT_PX : STRIP_PX, th = quarter ? QT_PX * vs : 8 * vs;
-    FusedWin fw;
-    memset(&fw, 0, sizeof fw);
-    fw.x = x;
-    fw.y = y;
-    fw.w = w;
-    fw.h = h;
-    fw.strip0 = x / tw;
-    fw.row0 = y / th;
-    if ( orient ) fw.m = *orient;
-    for ( int c = 0; c < 3; c++ ) {
-        const int dh = hs / comp[c].hs, dv = vs / comp[c].vs;
-        fw.bx0[c] = x / dh / 8;
-        fw.bx1[c] = (x + w - 1) / dh / 8 + 1;
-        fw.by0[c] = y / dv / 8;
-        fw.by1[c] = (y + h - 1) / dv / 8 + 1;
-    }
-    const dim3 grid((x + w - 1) / tw - fw.strip0 + 1, (y + h - 1) / th - fw.row0 + 1);
-    const size_t pitch = (size_t)(quarter ? h : w) * 3;
-    /* O: 0 = as stored, 1 = a half turn or a mirror, 2 = a quarter turn */
-    const int o = !orient ? 0 : quarter ? 2 : 1;
-    if ( hs == 1 && vs == 1 ) {
-#define GJ_K4W2(F, D, O) gj_launch_pdl(k_idct_rgb444<4, F, D, true, O>, grid, dim3(NT), 0, stream, d_coef, d_cext, comp[0].bcx, comp[0].nblk, d_out, width, height, pitch, prm, fw)
-#define GJ_K4W(F, D)                  \
-    do {                              \
-        if ( o == 0 ) GJ_K4W2(F, D, 0);  \
-        else if ( o == 1 ) GJ_K4W2(F, D, 1); \
-        else GJ_K4W2(F, D, 2);        \
-    } while ( 0 )
-        if ( idct_flavour == 0 && coef_dequantized ) GJ_K4W(0, false);
-        else if ( idct_flavour == 0 ) GJ_K4W(0, true);
-        else GJ_K4W(1, true);
-#undef GJ_K4W
-#undef GJ_K4W2
-        return cudaGetLastError() == cudaSuccess ? 0 : -1;
-    }
-    SsGrid sg;
-    ss_grid_rows(&sg, comp, 0, (comp[0].bcy + vs - 1) / vs, height);
-#define GJ_K4WS3(H, V, F, D, O) \
-    gj_launch_pdl(k_idct_rgb_ss<H, V, 4, F, D, true, O>, grid, dim3(TB * V + 2 * TB / H), 0, stream, d_coef, d_cext, sg, d_out, width, height, pitch, prm, fw)
-#define GJ_K4WS2(H, V, F, D)                   \
-    do {                                       \
-        if ( o == 0 ) GJ_K4WS3(H, V, F, D, 0);      \
-        else if ( o == 1 ) GJ_K4WS3(H, V, F, D, 1); \
-        else GJ_K4WS3(H, V, F, D, 2);               \
-    } while ( 0 )
-#define GJ_K4WS(H, V)                                                          \
-    do {                                                                       \
-        if ( idct_flavour == 0 && coef_dequantized ) GJ_K4WS2(H, V, 0, false); \
-        else if ( idct_flavour == 0 ) GJ_K4WS2(H, V, 0, true);                 \
-        else GJ_K4WS2(H, V, 1, true);                                          \
-    } while ( 0 )
-    if ( hs == 2 && vs == 2 ) GJ_K4WS(2, 2);
-    else if ( hs == 2 && vs == 1 ) GJ_K4WS(2, 1);
-    else if ( hs == 1 && vs == 2 ) GJ_K4WS(1, 2);
-    else return -1;
-#undef GJ_K4WS
-#undef GJ_K4WS2
-#undef GJ_K4WS3
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
-}
-
 /* ---- no colour transform: grey, planar and packed YCbCr formats ---- */
 static int sample_grid(SampleGrid* sg, const struct gj_raw_layout* raw, const struct gj_comp_geo* comp, int comp_count,
                        const uint8_t* comp_tbl)
@@ -1826,58 +1687,98 @@ static int block_win(BlockWin* bw, const struct gj_k4_window* win, int comp_coun
     return total;
 }
 
-extern "C" int gj_launch_idct_samples(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
-                                      const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int idct_flavour, int coef_dequantized,
-                                      const struct gj_dev_dec_tables* h_tables, const struct gj_k4_window* win, gj_stream_t stream)
+extern "C" int gj_launch_idct_fused(const struct gj_k4_plan* p, const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo comp[3],
+                                    const int comp_tq[3], uint8_t* d_out, int width, int height, int pitch, int my0, int my1,
+                                    const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
 {
-    IdctParams prm;
-    for ( int c = 0; c < GJ_MAX_COMP; c++ )
-        memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c < comp_count ? c : 0]], sizeof prm.q_zz[c]);
-    SampleGrid sg;
-    int total = sample_grid(&sg, raw, comp, comp_count, nullptr);
-    if ( total <= 0 ) return -1;
-    if ( idct_flavour != 0 && coef_dequantized ) return -1;
-    BlockWin bw;
-    memset(&bw, 0, sizeof bw);
-    if ( win && (total = block_win(&bw, win, comp_count)) <= 0 ) return -1;
-    const int grid = (total + SG_THREADS - 1) / SG_THREADS;
-#define GJ_K4S(F, D)                                                                                                                 \
-    do {                                                                                                                             \
-        if ( win ) k_idct_samples<F, D, true><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);          \
-        else k_idct_samples<F, D, false><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);               \
-    } while ( 0 )
-    if ( idct_flavour == 0 && coef_dequantized ) GJ_K4S(0, false);
-    else if ( idct_flavour == 0 ) GJ_K4S(0, true);
-    else if ( idct_flavour == GJ_IDCT_ISLOW ) GJ_K4S(GJ_IDCT_ISLOW, true);
-    else GJ_K4S(1, true);
-#undef GJ_K4S
+    const int hs = comp[0].hs, vs = comp[0].vs;
+    if ( comp[1].hs != 1 || comp[1].vs != 1 || comp[2].hs != 1 || comp[2].vs != 1 ) return -1;
+    if ( p->flavour != 0 && p->dequantize ) return -1;   // the float flavour needs raw coefficients
+    const int mcu_rows = (comp[0].bcy + vs - 1) / vs;
+    if ( my0 < 0 || my1 > mcu_rows || my0 >= my1 || (p->window && (my0 != 0 || my1 != mcu_rows)) ) return -1;
+    const IdctParams prm = idct_params(h_tables, comp_tq, 3);
+    FusedWin fw;
+    memset(&fw, 0, sizeof fw);
+    dim3 grid((comp[0].bcx + TB - 1) / TB, my1 - my0);
+    if ( p->window ) {   /* the rectangle of the image, into an image of its own size (turned: of the turned size) */
+        const int x = p->rect[0], y = p->rect[1], w = p->rect[2], h = p->rect[3];
+        if ( w < 1 || h < 1 || x < 0 || y < 0 || x + w > width || y + h > height ) return -1;
+        /* the pixels a CTA covers: a 512-pixel strip of an MCU row, or a quarter turn's 64 x 64 * vs tile */
+        const int tw = p->orient == 2 ? QT_PX : STRIP_PX, th = p->orient == 2 ? QT_PX * vs : 8 * vs;
+        fw.x = x;
+        fw.y = y;
+        fw.w = w;
+        fw.h = h;
+        fw.strip0 = x / tw;
+        fw.row0 = y / th;
+        if ( p->orient ) fw.m = p->map;
+        for ( int c = 0; c < 3; c++ ) {
+            const int dh = hs / comp[c].hs, dv = vs / comp[c].vs;
+            fw.bx0[c] = x / dh / 8;
+            fw.bx1[c] = (x + w - 1) / dh / 8 + 1;
+            fw.by0[c] = y / dv / 8;
+            fw.by1[c] = (y + h - 1) / dv / 8 + 1;
+        }
+        grid = dim3((x + w - 1) / tw - fw.strip0 + 1, (y + h - 1) / th - fw.row0 + 1);
+        pitch = (p->orient == 2 ? h : w) * 3;
+    }
+    else if ( p->flip == GJ_K4_FLIP_PITCH ) {   /* dec_opt_flipped: rows are written last to first */
+        d_out += (size_t)(height - 1) * (size_t)pitch;
+        pitch = -pitch;
+    }
+    /* the planes from the range's first block on, so that a frame can be transformed stripe by stripe */
+    SsGrid sg;
+    const int rows = ss_grid_rows(&sg, comp, my0, my1, height);
+    const size_t off = (size_t)my0 * comp[0].bcx;   // 4:4:4: the range's first block of every plane
+    d_out += (ptrdiff_t)my0 * 8 * vs * pitch;
+    auto launch = [&](auto H, auto V, auto VEC, auto F, auto RAW, auto WIN, auto O) {
+        /* the instances: raw coefficients for the float flavour, VEC 4 for the window ones, orientation only with a window */
+        if constexpr ( (F == 0 || RAW) && (WIN ? VEC == 4 : O == 0) ) {
+            if constexpr ( H == 1 && V == 1 )
+                gj_launch_pdl(k_idct_rgb444<VEC, F, RAW, WIN, O>, grid, dim3(NT), 0, stream, d_coef + off * 64, d_cext + off, comp[0].bcx,
+                              comp[0].nblk, d_out, width, rows, (size_t)pitch, prm, fw);
+            else
+                gj_launch_pdl(k_idct_rgb_ss<H, V, VEC, F, RAW, WIN, O>, grid, dim3(TB * V + 2 * TB / H), 0, stream, d_coef, d_cext, sg,
+                              d_out, width, rows, (size_t)pitch, prm, fw);
+            return 0;
+        }
+        return -1;
+    };
+    const int vec = p->window ? 4 : pick_vec(d_out, (size_t)pitch);
+    if ( instance(launch, std::tuple<>{}, OneOf<1, 2>{hs}, OneOf<1, 2>{vs}, OneOf<4, 1>{vec}, OneOf<0, 1>{p->flavour},
+                  OneOf<false, true>{!p->dequantize}, OneOf<false, true>{p->window}, OneOf<0, 1, 2>{p->orient}) )
+        return -1;
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
-extern "C" int gj_launch_idct_scaled(const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp, int comp_count,
-                                     const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw, int n,
-                                     const struct gj_dev_dec_tables* h_tables, const struct gj_k4_window* win, gj_stream_t stream)
+extern "C" int gj_launch_idct_blocks(const struct gj_k4_plan* p, const int16_t* d_coef, const uint8_t* d_cext, const struct gj_comp_geo* comp,
+                                     int comp_count, const int* comp_tq, uint8_t* d_raw, const struct gj_raw_layout* raw,
+                                     const struct gj_dev_dec_tables* h_tables, gj_stream_t stream)
 {
-    IdctParams prm;
-    for ( int c = 0; c < GJ_MAX_COMP; c++ )
-        memcpy(prm.q_zz[c], h_tables->qinv_zz[comp_tq[c < comp_count ? c : 0]], sizeof prm.q_zz[c]);
+    const IdctParams prm = idct_params(h_tables, comp_tq, comp_count);
     SampleGrid sg;
     int total = sample_grid(&sg, raw, comp, comp_count, nullptr);
     if ( total <= 0 ) return -1;
+    if ( p->flavour != 0 && p->dequantize ) return -1;
     BlockWin bw;
     memset(&bw, 0, sizeof bw);
-    if ( win && (total = block_win(&bw, win, comp_count)) <= 0 ) return -1;
+    if ( p->window && (total = block_win(&bw, &p->win, comp_count)) <= 0 ) return -1;
     const int grid = (total + SG_THREADS - 1) / SG_THREADS;
-#define GJ_K4R(N)                                                                                                                    \
-    do {                                                                                                                             \
-        if ( win ) k_idct_scaled<N, true><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);              \
-        else k_idct_scaled<N, false><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);                   \
-    } while ( 0 )
-    if ( n == 4 ) GJ_K4R(4);
-    else if ( n == 2 ) GJ_K4R(2);
-    else if ( n == 1 ) GJ_K4R(1);
-    else return -1;
-#undef GJ_K4R
+    auto samples = [&](auto F, auto RAW, auto WIN) {
+        if constexpr ( F == 0 || RAW ) {   // (the float flavour and ISLOW read raw coefficients)
+            k_idct_samples<F, RAW, WIN><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);
+            return 0;
+        }
+        return -1;
+    };
+    auto scaled = [&](auto N, auto WIN) {
+        k_idct_scaled<N, WIN><<<grid, SG_THREADS, 0, stream>>>(d_coef, d_cext, sg, total, d_raw, prm, bw);
+        return 0;
+    };
+    if ( p->kernel == GJ_K4_SCALED ? instance(scaled, std::tuple<>{}, OneOf<4, 2, 1>{p->n}, OneOf<false, true>{p->window})
+                                   : instance(samples, std::tuple<>{}, OneOf<0, 1, GJ_IDCT_ISLOW>{p->flavour},
+                                              OneOf<false, true>{!p->dequantize}, OneOf<false, true>{p->window}) )
+        return -1;
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
