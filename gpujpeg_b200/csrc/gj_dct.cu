@@ -5,7 +5,8 @@
  *       = colour transform + component split + 8x8 forward DCT + quantisation in ONE pass over HBM
  *       (the reference runs a preprocessor kernel and three DCT launches with a planar u8 round trip
  *        in between: src/gpujpeg_preprocessor.cu:163-201, src/gpujpeg_dct_gpu.cu:180-294).
- *       Algorithmic traffic: 3 B read + 6 B written per pixel.
+ *       Algorithmic traffic: 3 B read + at most 6 B written per pixel: of every block only the chunks the Huffman
+ *       coders read (gj_coef_live_chunks), rounded up to 32-byte sectors.
  *
  *   K4  k_idct_rgb444 : int16 zig-zag coefficients -> RGB u8 interleaved
  *       = (dequantisation +) inverse DCT + level shift + colour transform + interleave in one pass
@@ -21,7 +22,8 @@
  * phase every thread handles 4 pixels = 12 interleaved bytes = three 32-bit words, read from / written
  * to global memory directly (a warp touches 384 contiguous bytes); the only shared-memory traffic is
  * the planar staging area between the two phases.  No conversion-pipe (XU) instruction is used for
- * the colour transform (see gj_device.cuh); clamping + byte packing use cvt.pack.sat (I2IP).
+ * the colour transform (integer dot products, gj_rgb4_to_ycbcr in gj_device.cuh); clamping + byte packing use
+ * cvt.pack.sat (I2IP).
  */
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -46,6 +48,9 @@ constexpr int BLK_F = 68;              // floats per block in K1's planar stagin
                                        // distinct bank groups)
 constexpr int K1_SMEM = 3 * TB * BLK_F * 4;   // 52224 B
 constexpr int K1_OUT_STRIDE = 9;              // uint4 per block slot of K1's output staging (8 + 1 pad: 144-byte stride)
+/* CTAs of nt threads (one planar staging block each) that the shared memory of an SM holds: 228 KB, 1 KB of it reserved
+ * per CTA.  The subsampled K1's register budget is held to it (4:2:0: 4 CTAs, 80 registers). */
+constexpr int k1_ctas_per_sm(int nt) { return 228 * 1024 / (nt * BLK_F * 4 + 1024); }
 constexpr int K4_PLANE = 8 * STRIP_PX;        // bytes per component plane of a strip
 
 struct FdctParams {
@@ -97,10 +102,52 @@ __device__ __forceinline__ void quantise_store(const float (&v)[64], const float
         dst[i] = make_uint4(packed[4 * i], packed[4 * i + 1], packed[4 * i + 2], packed[4 * i + 3]);
 }
 
+/* colour transform of a 4-pixel group (three loaded words) of which `left` >= 1 pixels lie inside the image; pixels
+ * outside the image are 0 in every component */
+__device__ __forceinline__ void ycc4_clipped(uint32_t w0, uint32_t w1, uint32_t w2, int left, float4& y4, float4& cb4, float4& cr4)
+{
+    float y[4], cb[4], cr[4];
+    gj_rgb4_to_ycbcr(w0, w1, w2, y, cb, cr);
+    y4 = make_float4(y[0], y[1], y[2], y[3]);
+    cb4 = make_float4(cb[0], cb[1], cb[2], cb[3]);
+    cr4 = make_float4(cr[0], cr[1], cr[2], cr[3]);
+    if ( left < 4 ) {   // the image ends inside this group
+        if ( left <= 1 ) { y4.y = cb4.y = cr4.y = 0.f; }
+        if ( left <= 2 ) { y4.z = cb4.z = cr4.z = 0.f; }
+        if ( left <= 3 ) { y4.w = cb4.w = cr4.w = 0.f; }
+    }
+}
+
+/* A thread's quantised block into its slot of the output staging area: only the chunks the coefficient buffer keeps
+ * (gj_coef_live_chunks), rounded up to whole 32-byte sectors (half-written sectors made K1 3 us slower at 8K, DESIGN §6),
+ * their number next to the slots for the line stores that follow. */
+__device__ __forceinline__ void stage_live_block(uint4* s_out, uint8_t* s_live, int slot, uint64_t nz, const uint32_t (&packed)[32])
+{
+    const int live = (gj_coef_live_chunks(nz) + 1) & ~1;
+    s_live[slot] = (uint8_t)live;
+#pragma unroll
+    for ( int i = 0; i < 8; i++ )
+        if ( i < live ) s_out[slot * K1_OUT_STRIDE + i] = make_uint4(packed[4 * i], packed[4 * i + 1], packed[4 * i + 2], packed[4 * i + 3]);
+}
+
+/* The thread's eight chunks of the line stores (chunk k: slot (threadIdx.x + k * nt) / 8, part threadIdx.x % 8) and the live
+ * chunk counts of their slots, all loaded before the first store: a load behind each store's condition would put two
+ * shared-memory round trips in front of every store. */
+__device__ __forceinline__ void load_staged(const uint4* s_out, const uint8_t* s_live, int nt, uint4 (&chunk)[8], int (&live)[8])
+{
+#pragma unroll
+    for ( int k = 0; k < 8; k++ ) {
+        const int q = threadIdx.x + k * nt;
+        chunk[k] = s_out[(q >> 3) * K1_OUT_STRIDE + (q & 7)];
+        live[k] = s_live[q >> 3];
+    }
+}
+
 /* =========================================================================================== */
 /* K1                                                                                            */
 
 // VEC = 4: base pointer and pitch are 4-byte aligned -> 32-bit global loads; VEC = 1: byte loads
+// 80 registers without a bound: 4 CTAs per SM (with k1_ctas_per_sm(NT) as the bound ptxas spills 8 bytes)
 template <int VEC>
 __global__ void __launch_bounds__(NT)
 k_fdct_rgb444(const uint8_t* __restrict__ raw, int width, int height, size_t pitch, int16_t* __restrict__ coef,
@@ -155,18 +202,8 @@ k_fdct_rgb444(const uint8_t* __restrict__ raw, int width, int height, size_t pit
         if ( g >= GROUPS ) break;
         const int row = g >> 7, gx = g & 127, px0 = gx * 4;
         float4 y4 = make_float4(0.f, 0.f, 0.f, 0.f), cb4 = y4, cr4 = y4;
-        if ( row < vh && px0 < vw ) {
-            const uint32_t a0 = w0[it], a1 = w1[it], a2 = w2[it];
-            gj_rgb_to_ycbcr_m(gj_byte_as_magic(a0, 0), gj_byte_as_magic(a0, 1), gj_byte_as_magic(a0, 2), y4.x, cb4.x, cr4.x);
-            gj_rgb_to_ycbcr_m(gj_byte_as_magic(a0, 3), gj_byte_as_magic(a1, 0), gj_byte_as_magic(a1, 1), y4.y, cb4.y, cr4.y);
-            gj_rgb_to_ycbcr_m(gj_byte_as_magic(a1, 2), gj_byte_as_magic(a1, 3), gj_byte_as_magic(a2, 0), y4.z, cb4.z, cr4.z);
-            gj_rgb_to_ycbcr_m(gj_byte_as_magic(a2, 1), gj_byte_as_magic(a2, 2), gj_byte_as_magic(a2, 3), y4.w, cb4.w, cr4.w);
-            if ( px0 + 4 > vw ) {  // the image ends inside this group
-                if ( px0 + 1 >= vw ) { y4.y = cb4.y = cr4.y = 0.f; }
-                if ( px0 + 2 >= vw ) { y4.z = cb4.z = cr4.z = 0.f; }
-                if ( px0 + 3 >= vw ) { y4.w = cb4.w = cr4.w = 0.f; }
-            }
-        }
+        if ( row < vh && px0 < vw )
+            ycc4_clipped(w0[it], w1[it], w2[it], vw - px0, y4, cb4, cr4);
         const int off = (gx >> 1) * BLK_F + row * 8 + (gx & 1) * 4;
         *reinterpret_cast<float4*>(s_pl + off) = y4;
         *reinterpret_cast<float4*>(s_pl + TB * BLK_F + off) = cb4;
@@ -191,26 +228,30 @@ k_fdct_rgb444(const uint8_t* __restrict__ raw, int width, int height, size_t pit
     gj_fdct_block(v);
     /* quantise: q = rint(c * table) [ref: src/gpujpeg_dct_gpu.cu:276-283], zig-zag order.  The block (128 bytes) goes to
      * shared memory first and from there to the coefficient buffer as whole lines: a thread storing its own block
-     * straight away makes every store instruction of the warp touch 32 different lines, 16 bytes each. */
+     * straight away makes every store instruction of the warp touch 32 different lines, 16 bytes each.  Only the live
+     * chunks of a block are stored (gj_coef_live_chunks): the zero tail of a block is never read. */
     uint4* const s_out = reinterpret_cast<uint4*>(smem);   // slot = thread, K1_OUT_STRIDE uint4 apart (bank-conflict-free)
+    uint8_t* const s_live = smem + NT * K1_OUT_STRIDE * 16;
+    static_assert(NT * (K1_OUT_STRIDE * 16 + 1) <= K1_SMEM, "output staging must fit into the planar staging area");
     {
         uint32_t packed[32];
         const uint64_t nz = quantise_pack(v, prm.fwd_zz[comp == 0 ? 0 : 1], packed);
         const size_t bi = (size_t)comp * nblk + (size_t)by * bcx + bx0 + b;
         if ( active ) nzmask[bi] = nz;
-#pragma unroll
-        for ( int i = 0; i < 8; i++ )
-            s_out[threadIdx.x * K1_OUT_STRIDE + i] = make_uint4(packed[4 * i], packed[4 * i + 1], packed[4 * i + 2], packed[4 * i + 3]);
+        stage_live_block(s_out, s_live, threadIdx.x, nz, packed);
     }
     __syncthreads();
+    uint4 chunk[8];
+    int live[8];
+    load_staged(s_out, s_live, NT, chunk, live);
 #pragma unroll
     for ( int k = 0; k < 8; k++ ) {
         const int q = threadIdx.x + k * NT;
         const int slot = q >> 3, part = q & 7;
         const int c2 = slot >> 6, b2 = slot & 63;
-        if ( bx0 + b2 < bcx ) {
+        if ( bx0 + b2 < bcx && part < live[k] ) {
             const size_t bi = (size_t)c2 * nblk + (size_t)by * bcx + bx0 + b2;
-            reinterpret_cast<uint4*>(coef + bi * 64)[part] = s_out[slot * K1_OUT_STRIDE + part];
+            reinterpret_cast<uint4*>(coef + bi * 64)[part] = chunk[k];
         }
     }
 }
@@ -347,7 +388,7 @@ struct SsGrid {
 };
 
 template <int HS, int VS, int VEC>
-__global__ void __launch_bounds__(TB * VS + 2 * TB / HS)
+__global__ void __launch_bounds__(TB * VS + 2 * TB / HS, k1_ctas_per_sm(TB * VS + 2 * TB / HS))
 k_fdct_rgb_ss(const uint8_t* __restrict__ raw, int width, int height, size_t pitch, int16_t* __restrict__ coef,
               uint64_t* __restrict__ nzmask, const __grid_constant__ SsGrid grid, const __grid_constant__ FdctParams prm)
 {
@@ -400,18 +441,8 @@ k_fdct_rgb_ss(const uint8_t* __restrict__ raw, int width, int height, size_t pit
             if ( g >= GROUPS ) break;
             const int row = g >> 7, gx = g & 127, px0 = gx * 4;
             float4 y4 = make_float4(0.f, 0.f, 0.f, 0.f), cb4 = y4, cr4 = y4;
-            if ( row < vh && px0 < vw ) {
-                const uint32_t a0 = w0[it], a1 = w1[it], a2 = w2[it];
-                gj_rgb_to_ycbcr_m(gj_byte_as_magic(a0, 0), gj_byte_as_magic(a0, 1), gj_byte_as_magic(a0, 2), y4.x, cb4.x, cr4.x);
-                gj_rgb_to_ycbcr_m(gj_byte_as_magic(a0, 3), gj_byte_as_magic(a1, 0), gj_byte_as_magic(a1, 1), y4.y, cb4.y, cr4.y);
-                gj_rgb_to_ycbcr_m(gj_byte_as_magic(a1, 2), gj_byte_as_magic(a1, 3), gj_byte_as_magic(a2, 0), y4.z, cb4.z, cr4.z);
-                gj_rgb_to_ycbcr_m(gj_byte_as_magic(a2, 1), gj_byte_as_magic(a2, 2), gj_byte_as_magic(a2, 3), y4.w, cb4.w, cr4.w);
-                if ( px0 + 4 > vw ) {
-                    if ( px0 + 1 >= vw ) { y4.y = cb4.y = cr4.y = 0.f; }
-                    if ( px0 + 2 >= vw ) { y4.z = cb4.z = cr4.z = 0.f; }
-                    if ( px0 + 3 >= vw ) { y4.w = cb4.w = cr4.w = 0.f; }
-                }
-            }
+            if ( row < vh && px0 < vw )
+                ycc4_clipped(w0[it], w1[it], w2[it], vw - px0, y4, cb4, cr4);
             *reinterpret_cast<float4*>(s_y + (half * TB + (gx >> 1)) * BLK_F + row * 8 + (gx & 1) * 4) = y4;
             const int srow = half * 8 + row;           // row inside the strip
             if ( VS == 1 || (srow & 1) == 0 ) {
@@ -460,23 +491,26 @@ k_fdct_rgb_ss(const uint8_t* __restrict__ raw, int width, int height, size_t pit
     __syncthreads();   // the planes are in registers: their memory becomes the output staging area (see k_fdct_rgb444)
     gj_fdct_block(v);
     uint4* const s_out = reinterpret_cast<uint4*>(smem);
+    uint8_t* const s_live = smem + NTS * K1_OUT_STRIDE * 16;
+    static_assert(BLK_F * 4 >= K1_OUT_STRIDE * 16 + 1, "output staging must fit into the planar staging area (NTS blocks)");
     {
         uint32_t packed[32];
         const uint64_t nz = quantise_pack(v, prm.fwd_zz[comp == 0 ? 0 : 1], packed);
         if ( active ) nzmask[(size_t)grid.blk_off[comp] + (size_t)by * grid.bcx[comp] + bx] = nz;
-#pragma unroll
-        for ( int i = 0; i < 8; i++ )
-            s_out[threadIdx.x * K1_OUT_STRIDE + i] = make_uint4(packed[4 * i], packed[4 * i + 1], packed[4 * i + 2], packed[4 * i + 3]);
+        stage_live_block(s_out, s_live, threadIdx.x, nz, packed);
     }
     __syncthreads();
+    uint4 chunk[8];
+    int live[8];
+    load_staged(s_out, s_live, NTS, chunk, live);
 #pragma unroll
     for ( int k = 0; k < 8; k++ ) {
         const int q = threadIdx.x + k * NTS;
         const int slot = q >> 3, part = q & 7;
         int c2, bx2, by2;
-        if ( locate(slot, c2, bx2, by2) ) {
+        if ( part < live[k] && locate(slot, c2, bx2, by2) ) {
             const size_t bi = (size_t)grid.blk_off[c2] + (size_t)by2 * grid.bcx[c2] + bx2;
-            reinterpret_cast<uint4*>(coef + bi * 64)[part] = s_out[slot * K1_OUT_STRIDE + part];
+            reinterpret_cast<uint4*>(coef + bi * 64)[part] = chunk[k];
         }
     }
 }

@@ -1769,6 +1769,6 @@ GPUJPEG_API int gpujpegx_decoder_run_resident(struct gpujpeg_decoder* d, uint8_t
 GPUJPEG_API int gpujpegx_decoder_get_coefficients(struct gpujpeg_decoder* d, int16_t* out, size_t count)
 {
     if ( !d || !d->initialised || !d->last_valid || count != d->geo.coef_count ) return -1;
-    if ( gj_coef_to_host_natural(d->d_coef, d->d_cext, count, out, d->stream) ) return -1;
+    if ( gj_coef_to_host_natural(d->d_coef, d->d_cext, NULL, count, out, d->stream) ) return -1;
     return d->k4.dequantize;
 }

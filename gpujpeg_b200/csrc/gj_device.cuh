@@ -79,6 +79,22 @@ GJ_HD int gj_cext_of(int last_zz) { return (last_zz >> 3) + 1; }
 /* is zig-zag coefficient k of a block with extent ext stored in the coefficient buffer?  (otherwise it is zero) */
 GJ_HD bool gj_cext_holds(int ext, int k) { return (k >> 3) < ext; }
 
+/* The encoder's coefficient buffer holds of every block the 16-byte chunks below gj_coef_live_chunks of its non-zero mask
+ * (bit k <=> zig-zag coefficient k != 0): chunks 0 and 1 always (the Huffman coders load the first 16 coefficients of every
+ * block unconditionally), chunk c >= 2 if the block has a non-zero coefficient at zig-zag index >= 8c.  The rest of the
+ * buffer is undefined: a reader takes coefficient k >= 16 only where bit k of the mask is set, or zero past the chunks. */
+GJ_HD int gj_coef_live_chunks(uint64_t nz)
+{
+#if defined(__CUDA_ARCH__)
+    const int last = 63 - __clzll((long long)nz);   /* -1 for an all-zero block */
+#else
+    int last = -1;
+    for ( int k = 0; k < 64; k++ )
+        if ( (nz >> k) & 1u ) last = k;
+#endif
+    return last < 16 ? 2 : (last >> 3) + 1;
+}
+
 #if defined(__CUDACC__)
 /* the 64 zig-zag coefficients of a block as 32 packed int16 pairs: chunks below the extent from the buffer, the rest zero.
  * The loop is unrolled, so the register layout is that of a whole-block load. */
@@ -104,7 +120,8 @@ __device__ __forceinline__ void gj_load_coef_block(const int16_t* __restrict__ b
  *   - floor((S+128)/256) is obtained by adding 1.5*2^23 to S/256 + 2^-9: the add rounds to the nearest
  *     integer, and S/256 + 2^-9 is never a tie and never crosses the next integer (fractions are
  *     k/256 - 127.5/256), so the rounded value IS the arithmetic shift of the reference.
- * tests/test_kernel_math.py checks all 2^24 RGB inputs against the integer definition. */
+ * tests/test_kernel_math.py checks all 2^24 RGB inputs against the integer definition.  k_fdct_rgb444_bulk uses it;
+ * k_fdct_rgb444 and k_fdct_rgb_ss take the integer evaluation gj_rgb4_to_ycbcr below. */
 #define GJ_MAGIC23 8388608.0f   /* 2^23     : integer <-> float mantissa trick for bytes   */
 #define GJ_MAGIC15 12582912.0f  /* 1.5*2^23 : round-to-nearest-integer by addition         */
 GJ_HD float gj_byte_as_magic(uint32_t word, int i)
@@ -132,6 +149,89 @@ GJ_HD void gj_rgb_to_ycbcr_m(float rm, float gm, float bm, float& y, float& cb, 
 GJ_HD void gj_rgb_to_ycbcr(float r, float g, float b, float& y, float& cb, float& cr)
 {
     gj_rgb_to_ycbcr_m(r + GJ_MAGIC23, g + GJ_MAGIC23, b + GJ_MAGIC23, y, cb, cr);
+}
+
+/* The same transform evaluated as the reference's integers, on four pixels at once: the three little-endian words
+ * w0 = r0 g0 b0 r1, w1 = g1 b1 r2 g2, w2 = b2 r3 g3 b3 that K1 loads.  With s = c + (c == 255) per channel,
+ *     Y  = min((77 sR + 150 sG + 29 sB + 128) >> 8, 255)
+ *     Cb = min((32896 - T) >> 8, 255),  T = 43 sR + 85 sG - 128 sB
+ *     Cr = min((32896 - T) >> 8, 255),  T = -128 sR + 107 sG + 21 sB
+ * Each sum is two byte dot products (DP4A): one over the pixel's bytes and one over its (c == 255) bytes, 0 or 1, which
+ * adds the c*256/255 correction.  T's coefficients fit in a signed byte, 128 does not: hence Cb and Cr as 32896 - T.
+ * The result becomes a float without a conversion instruction: the shifted sum is added into the mantissa of 2^23,
+ * clamped in float and 2^23 subtracted (for Cb and Cr the sum is negated on the way: the accumulator holds
+ * -S - 1 = T - 32897, whose arithmetic shift is -1 - (S >> 8)).  About 19 instructions per pixel instead of 30.
+ * tests/test_k1_live_chunks.py checks all 2^24 RGB inputs against the integer definition. */
+GJ_HD uint32_t gj_prmt(uint32_t a, uint32_t b, uint32_t sel)
+{
+#if defined(__CUDA_ARCH__)
+    return __byte_perm(a, b, sel);
+#else
+    const uint64_t x = (uint64_t)b << 32 | a;
+    uint32_t d = 0;
+    for ( int i = 0; i < 4; i++ )
+        d |= (uint32_t)((x >> (8 * ((sel >> (4 * i)) & 7u))) & 0xFFu) << (8 * i);
+    return d;
+#endif
+}
+/* c + a.b over the four bytes: a unsigned, b unsigned (uu) or signed (us) */
+GJ_HD int gj_dp4a_uu(uint32_t a, uint32_t b, int c)
+{
+#if defined(__CUDA_ARCH__)
+    int d;
+    asm("dp4a.u32.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
+    return d;
+#else
+    for ( int i = 0; i < 4; i++ )
+        c += (int)((a >> (8 * i)) & 0xFFu) * (int)((b >> (8 * i)) & 0xFFu);
+    return c;
+#endif
+}
+GJ_HD int gj_dp4a_us(uint32_t a, uint32_t b, int c)
+{
+#if defined(__CUDA_ARCH__)
+    int d;
+    asm("dp4a.u32.s32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
+    return d;
+#else
+    for ( int i = 0; i < 4; i++ )
+        c += (int)((a >> (8 * i)) & 0xFFu) * (int)(int8_t)((b >> (8 * i)) & 0xFFu);
+    return c;
+#endif
+}
+GJ_HD float gj_bits_float(uint32_t u)
+{
+#if defined(__CUDA_ARCH__)
+    return __uint_as_float(u);
+#else
+    union { uint32_t u; float f; } c;
+    c.u = u;
+    return c.f;
+#endif
+}
+/* 1 in every byte of w that is 255, 0 in the others (bit 7 of (c & 127) + 1 is set iff c & 127 == 127) */
+GJ_HD uint32_t gj_eq255_4(uint32_t w) { return (((w & 0x7F7F7F7Fu) + 0x01010101u) & w & 0x80808080u) >> 7; }
+/* one pixel: p holds its bytes r g b at byte offset `at` (0 or 1), m the (c == 255) bytes at the same places */
+template <int at>
+GJ_HD void gj_ycc_int_px(uint32_t p, uint32_t m, float& y, float& cb, float& cr)
+{
+    constexpr uint32_t KY = (77u | 150u << 8 | 29u << 16) << (8 * at);
+    constexpr uint32_t KCB = (43u | 85u << 8 | 0x80u << 16) << (8 * at);    /* 43, 85, -128 */
+    constexpr uint32_t KCR = (0x80u | 107u << 8 | 21u << 16) << (8 * at);   /* -128, 107, 21 */
+    const int sy = gj_dp4a_uu(m, KY, gj_dp4a_uu(p, KY, 128));
+    const int tb = gj_dp4a_us(m, KCB, gj_dp4a_us(p, KCB, -32897));
+    const int tr = gj_dp4a_us(m, KCR, gj_dp4a_us(p, KCR, -32897));
+    y = fminf(gj_bits_float((uint32_t)(sy >> 8) + 0x4B000000u), GJ_MAGIC23 + 255.0f) - GJ_MAGIC23;
+    cb = (GJ_MAGIC23 + 511.0f) - fmaxf(gj_bits_float((uint32_t)((tb >> 8) + 0x4B000200)), GJ_MAGIC23 + 256.0f);
+    cr = (GJ_MAGIC23 + 511.0f) - fmaxf(gj_bits_float((uint32_t)((tr >> 8) + 0x4B000200)), GJ_MAGIC23 + 256.0f);
+}
+GJ_HD void gj_rgb4_to_ycbcr(uint32_t w0, uint32_t w1, uint32_t w2, float (&y)[4], float (&cb)[4], float (&cr)[4])
+{
+    const uint32_t m0 = gj_eq255_4(w0), m1 = gj_eq255_4(w1), m2 = gj_eq255_4(w2);
+    gj_ycc_int_px<0>(w0, m0, y[0], cb[0], cr[0]);
+    gj_ycc_int_px<0>(gj_prmt(w0, w1, 0x6543), gj_prmt(m0, m1, 0x6543), y[1], cb[1], cr[1]);
+    gj_ycc_int_px<0>(gj_prmt(w1, w2, 0x5432), gj_prmt(m1, m2, 0x5432), y[2], cb[2], cr[2]);
+    gj_ycc_int_px<1>(w2, m2, y[3], cb[3], cr[3]);
 }
 
 /* YCbCr (JPEG full range) -> RGB, integer [ref: src/gpujpeg_colorspace.h:86-101, 268-283]:

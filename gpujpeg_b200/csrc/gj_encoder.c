@@ -1313,5 +1313,5 @@ GPUJPEG_API long long gpujpegx_encoder_get_stream(struct gpujpeg_encoder* e, uin
 GPUJPEG_API int gpujpegx_encoder_get_coefficients(struct gpujpeg_encoder* e, int16_t* out, size_t count)
 {
     if ( !e || !e->initialised || count != e->geo.coef_count ) return -1;
-    return gj_coef_to_host_natural(e->d_coef, NULL, count, out, e->stream);
+    return gj_coef_to_host_natural(e->d_coef, NULL, e->d_nzmask, count, out, e->stream);
 }

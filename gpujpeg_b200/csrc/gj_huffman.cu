@@ -1533,18 +1533,21 @@ __global__ void __launch_bounds__(256) k_rst_check(const __grid_constant__ gj_hu
     if ( s > 0 && a.d_list_code[a.first_rank[scan] + (uint32_t)s - 1u] != (uint8_t)(0xD0 + ((s - 1) & 7)) ) atomicExch(a.d_error, 1u);
 }
 
-/* zig-zag device coefficients -> natural order (debug / parity-test path only) */
+/* zig-zag device coefficients -> natural order (debug / parity-test path only).  Blocks are read as far as the coefficient
+ * buffer holds them: the decoder's up to its extent byte (cext), the encoder's up to the live chunks of its non-zero mask
+ * (nzmask, gj_coef_live_chunks); zero beyond.  Without either the blocks are whole. */
 __constant__ uint8_t c_zz2nat[64] = {
     0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
     41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
     30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
-__global__ void k_coef_to_natural(const int16_t* __restrict__ in, const uint8_t* __restrict__ cext, int16_t* __restrict__ out,
-                                  size_t nblocks)
+__global__ void k_coef_to_natural(const int16_t* __restrict__ in, const uint8_t* __restrict__ cext,
+                                  const uint64_t* __restrict__ nzmask, int16_t* __restrict__ out, size_t nblocks)
 {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if ( i >= nblocks * 64 ) return;
     const int k = (int)(i & 63);
-    out[(i & ~(size_t)63) + c_zz2nat[k]] = !cext || gj_cext_holds(cext[i >> 6], k) ? in[i] : (int16_t)0;
+    const bool held = cext ? gj_cext_holds(cext[i >> 6], k) : nzmask ? (k >> 3) < gj_coef_live_chunks(nzmask[i >> 6]) : true;
+    out[(i & ~(size_t)63) + c_zz2nat[k]] = held ? in[i] : (int16_t)0;
 }
 
 }  // namespace
@@ -1804,12 +1807,13 @@ extern "C" int gj_launch_huffman_decode(const struct gj_huff_dec_args* a, gj_str
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
-extern "C" int gj_coef_to_host_natural(const int16_t* d_coef, const uint8_t* d_cext, size_t count, int16_t* h_out, gj_stream_t stream)
+extern "C" int gj_coef_to_host_natural(const int16_t* d_coef, const uint8_t* d_cext, const uint64_t* d_nzmask, size_t count,
+                                       int16_t* h_out, gj_stream_t stream)
 {
     int16_t* d_tmp = nullptr;
     if ( cudaMalloc(&d_tmp, count * sizeof(int16_t)) != cudaSuccess ) return -1;
     const size_t nblocks = count / 64;
-    k_coef_to_natural<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(d_coef, d_cext, d_tmp, nblocks);
+    k_coef_to_natural<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(d_coef, d_cext, d_nzmask, d_tmp, nblocks);
     cudaMemcpyAsync(h_out, d_tmp, count * sizeof(int16_t), cudaMemcpyDeviceToHost, stream);
     const cudaError_t e = cudaStreamSynchronize(stream);
     cudaFree(d_tmp);

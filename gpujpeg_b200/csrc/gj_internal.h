@@ -731,8 +731,9 @@ int gj_encoder_setup_coefficients(struct gpujpeg_encoder* e, const struct gpujpe
 int gj_encoder_finish(struct gpujpeg_encoder* e, uint8_t** out, size_t* out_size);
 
 /* debug/test helper: device coefficient buffer (zig-zag) -> host natural order, block-major; coefficients past a block's
- * extent read as zero (d_cext NULL: every block is whole, as the encoder's) */
-int gj_coef_to_host_natural(const int16_t* d_coef, const uint8_t* d_cext, size_t count, int16_t* h_out, gj_stream_t stream);
+ * extent read as zero: the decoder's extent bytes d_cext, or the encoder's non-zero masks d_nzmask (gj_coef_live_chunks) */
+int gj_coef_to_host_natural(const int16_t* d_coef, const uint8_t* d_cext, const uint64_t* d_nzmask, size_t count, int16_t* h_out,
+                            gj_stream_t stream);
 
 /* thin wrappers over the CUDA runtime so the host files stay plain C without cuda headers */
 int gj_cuda_malloc(void** p, size_t size);
