@@ -423,11 +423,12 @@ class Transcoder:
     """gpujpegx_transcoder_*: lossless JPEG-to-JPEG rewrite on the GPU (include/gpujpegx.h) -- the same quantised coefficients as
     one baseline frame with the restart interval and Huffman tables asked for, optionally turned and mirrored"""
 
-    def __init__(self, stream=0, transform="none", restart="auto", huffman="standard", perfect=False):
+    def __init__(self, stream=0, transform="none", restart="auto", huffman="standard", perfect=False, crop=None):
         """transform: "none", "auto" (the stream's SPIFF / Exif orientation) or "0" / "90" / "180" / "270", optionally followed by
         "-" -- turn clockwise, then mirror horizontally (tran_opt_transform).  restart: "auto" or the interval in MCUs (0: no
         markers).  huffman: "standard" (Annex K) or "optimized" (fitted to the frame).  perfect: refuse frames whose partial edge
-        iMCUs would move instead of dropping them."""
+        iMCUs would move instead of dropping them.  crop: None or (x, y, w, h) of the transformed image, its origin rounded down
+        to the output's iMCU grid (tran_opt_crop, jpegtran -crop)."""
         self._h = lib.gpujpegx_transcoder_create(C.c_void_p(stream))
         if not self._h:
             raise GpuJpegError("gpujpegx_transcoder_create failed (no CUDA device?)")
@@ -435,6 +436,9 @@ class Transcoder:
         self.set_option("tran_opt_restart", str(restart))
         self.set_option("tran_opt_huffman", huffman)
         self.set_option("tran_opt_perfect", "1" if perfect else "0")
+        if crop is not None:
+            x, y, w, h = (int(v) for v in crop)
+            self.set_option("tran_opt_crop", "%dx%d+%d+%d" % (w, h, x, y))
 
     def set_option(self, key, val):
         if lib.gpujpegx_transcoder_set_option(self._h, key.encode(), val.encode()) != 0:

@@ -258,6 +258,21 @@ int gj_parse_orientation(const char* val, int* mode, int* rot, int* flip)
     return -1;
 }
 
+int gj_parse_crop(const char* p, int v[4])
+{
+    static const char seps[4] = {'x', '+', '+', 0};
+    for ( int i = 0; i < 4; i++ ) {
+        long n = 0;
+        const char* q = p;
+        while ( *q >= '0' && *q <= '9' && n < (1L << 30) )
+            n = n * 10 + (*q++ - '0');
+        if ( q == p || n >= (1L << 30) || *q != seps[i] ) return -1;
+        v[i] = (int)n;
+        p = q + 1;
+    }
+    return v[0] >= 1 && v[1] >= 1 ? 0 : -1;
+}
+
 int gj_orient_frame(int w, int h, int rot, int flip, const int* crop, int* ow, int* oh, struct gj_orient_map* m, int src[4])
 {
     rot &= 3;
@@ -373,6 +388,66 @@ int gj_transcode_plan(int w, int h, int comp_count, const int* hs_in, const int*
         b->vis_by = lim_oy < b->out_bcy ? lim_oy : b->out_bcy;
     }
     return 0;
+}
+
+int gj_transcode_crop(const struct gj_transcode_plan* full, int w, int h, int comp_count, int out_interleaved, const int rect[4],
+                      struct gj_transcode_plan* pl, char* why)
+{
+    const int wu = full->transpose ? h : w, hu = full->transpose ? w : h;   /* transformed, before the trim */
+    const int x = rect[0], y = rect[1], cw = rect[2], ch = rect[3];
+    if ( cw < 1 || ch < 1 || x < 0 || y < 0 || x >= wu || y >= hu || cw > wu - x || ch > hu - y ) {
+        snprintf(why, GJ_WHY_BYTES, "the crop %dx%d+%d+%d does not lie inside the %dx%d transformed image", cw, ch, x, y, wu, hu);
+        return -1;
+    }
+    int max_h = 1, max_v = 1;
+    for ( int c = 0; c < comp_count; c++ ) {
+        if ( full->hs[c] > max_h ) max_h = full->hs[c];
+        if ( full->vs[c] > max_v ) max_v = full->vs[c];
+    }
+    /* the origin on the output's iMCU grid: whole iMCUs are what moves without re-encoding */
+    const int imcu_w = 8 * max_h, imcu_h = 8 * max_v;
+    const int x0 = x - x % imcu_w, y0 = y - y % imcu_h;
+    if ( x0 >= full->width || y0 >= full->height ) {
+        snprintf(why, GJ_WHY_BYTES, "the crop %dx%d+%d+%d starts in the partial edge iMCUs the transform drops (%dx%d remain)", cw, ch, x,
+                 y, full->width, full->height);
+        return -1;
+    }
+    *pl = *full;
+    pl->width = (x + cw < full->width ? x + cw : full->width) - x0;
+    pl->height = (y + ch < full->height ? y + ch : full->height) - y0;
+    struct gj_geometry go;
+    plan_geometry(&go, pl->width, pl->height, comp_count, pl->hs, pl->vs, out_interleaved);
+    for ( int c = 0; c < comp_count; c++ ) {
+        const struct gj_blk_map* f = &full->blk[c];
+        struct gj_blk_map* b = &pl->blk[c];
+        const int bx = x0 / imcu_w * pl->hs[c], by = y0 / imcu_h * pl->vs[c];   /* the origin in the component's blocks */
+        b->ax0 = f->ax0 + f->axx * bx + f->axy * by;
+        b->ay0 = f->ay0 + f->ayx * bx + f->ayy * by;
+        b->out_bcx = go.comp[c].bcx;
+        b->out_bcy = go.comp[c].bcy;
+        /* source blocks along the output's x / y: a reversed axis starts at its last kept block (gj_transcode_plan) */
+        const int lim_x = full->neg_x ? f->ax0 + 1 : f->src_bcx, lim_y = full->neg_y ? f->ay0 + 1 : f->src_bcy;
+        const int lim_ox = (full->transpose ? lim_y : lim_x) - bx, lim_oy = (full->transpose ? lim_x : lim_y) - by;
+        b->vis_bx = lim_ox < b->out_bcx ? lim_ox : b->out_bcx;
+        b->vis_by = lim_oy < b->out_bcy ? lim_oy : b->out_bcy;
+    }
+    return 0;
+}
+
+void gj_transcode_window(const struct gj_transcode_plan* pl, int comp_count, struct gj_blk_rect win[GJ_MAX_COMP])
+{
+    memset(win, 0, sizeof(struct gj_blk_rect) * GJ_MAX_COMP);
+    for ( int c = 0; c < comp_count; c++ ) {
+        const struct gj_blk_map* b = &pl->blk[c];
+        /* the visible blocks' corners; a dummy reads a block of the visible edge */
+        const int xa = b->ax0, ya = b->ay0;
+        const int xb = b->axx * (b->vis_bx - 1) + b->axy * (b->vis_by - 1) + b->ax0;
+        const int yb = b->ayx * (b->vis_bx - 1) + b->ayy * (b->vis_by - 1) + b->ay0;
+        win[c].bx0 = xa < xb ? xa : xb;
+        win[c].by0 = ya < yb ? ya : yb;
+        win[c].bx1 = (xa < xb ? xb : xa) + 1;
+        win[c].by1 = (ya < yb ? yb : ya) + 1;
+    }
 }
 
 size_t gj_com_segments(const uint8_t* d, size_t size, uint8_t* out)

@@ -130,6 +130,9 @@ struct gpujpeg_decoder {
     uint8_t coef_qt[GJ_MAX_COMP][64];
     int coef_tq[GJ_MAX_COMP];
     uint8_t* com; size_t com_cap;
+    /* ... and the caller's window over the frame's blocks (gj_coef_window_fn; NULL: every block) */
+    gj_coef_window_fn coef_window;
+    void* coef_window_ctx;
 };
 
 /* ---- output descriptor helpers [ref: src/gpujpeg_decoder.c:44-92] ---- */
@@ -881,6 +884,17 @@ static int grow_pick(struct gpujpeg_decoder* d, size_t pairs)
     return grow_dev((void**)&d->d_pick, &d->d_pick_size, pairs * 8);
 }
 
+/* gj_decoder_decode_coefficients with a window: the caller's rectangle of blocks on the frame's geometry, decoded as a
+ * dec_opt_crop frame decodes the blocks K4 needs (the same pick lists, the same kernels, the same extent rule) */
+static int coef_window(struct gpujpeg_decoder* d, const struct gj_stream* st)
+{
+    if ( !d->coef_only || !d->coef_window ) return 0;
+    const int r = d->coef_window(d->coef_window_ctx, &d->geo, st->progressive, &st->metadata, d->k4.win.blk);
+    if ( r < 0 ) return -1;
+    d->crop = r;
+    return 0;
+}
+
 /* Progressive (SOF2) frames, from the first SOS on: the same upload, K0 and host marker walk as a baseline frame, then per
  * scan the parameters and Huffman tables (those in force at its SOS), one table upload, the scan kernels in stream order
  * (gj_progressive.cu) and the same K4 / output stage.  Segment-info tables and dec_opt_huffman / dec_opt_huffman_lanes do not
@@ -932,6 +946,7 @@ static int decode_progressive(struct gpujpeg_decoder* d, uint8_t* image, size_t 
         if ( !d->coef_only && size_output(d, pi) ) return GPUJPEG_ERROR;
     }
     const struct gj_geometry* g = &d->geo;
+    if ( coef_window(d, st) ) return GPUJPEG_ERROR;
 
     /* scans and their Huffman tables */
     int nlut = 0;
@@ -1232,6 +1247,7 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     if ( !d->coef_only && (((d->k4.kernel != GJ_K4_FUSED || d->crop) && gj_raw_layout_init(&d->raw, &pi)) || size_output(d, &pi)) )
         return GPUJPEG_ERROR;
     const struct gj_geometry* g = &d->geo;
+    if ( !st.progressive && coef_window(d, &st) ) return GPUJPEG_ERROR;
 
     if ( st.progressive ) return decode_progressive(d, image, image_size, output, &st, &p, &pi, &k4, pos, adobe, early_cs, stats, t_begin);
 
@@ -1478,14 +1494,19 @@ int gpujpeg_decoder_decode(struct gpujpeg_decoder* d, uint8_t* image, size_t ima
     return GPUJPEG_NOERR;
 }
 
-int gj_decoder_decode_coefficients(struct gpujpeg_decoder* d, const uint8_t* image, size_t image_size, struct gj_coef_frame* f)
+int gj_decoder_decode_coefficients(struct gpujpeg_decoder* d, const uint8_t* image, size_t image_size, gj_coef_window_fn window,
+                                   void* ctx, struct gj_coef_frame* f)
 {
     if ( !d || !image || !f ) return -1;
     struct gpujpeg_decoder_output output;
     gpujpeg_decoder_output_set_default(&output);
     d->coef_only = 1;
+    d->coef_window = window;
+    d->coef_window_ctx = ctx;
     const int rc = gpujpeg_decoder_decode(d, (uint8_t*)image, image_size, &output);
     d->coef_only = 0;
+    d->coef_window = NULL;
+    d->coef_window_ctx = NULL;
     d->last_valid = 0;   /* a resident re-run would take the raw coefficients for K4's */
     if ( rc ) return -1;
     const size_t com = gj_com_segments(image, image_size, NULL);
@@ -1578,22 +1599,6 @@ int gpujpeg_decoder_get_image_info(uint8_t* image, size_t image_size, struct gpu
     return 0;
 }
 
-/* djpeg's -crop syntax "WxH+X+Y", decimal: v = {W, H, X, Y}; 0 on success */
-static int parse_crop(const char* p, int v[4])
-{
-    static const char seps[4] = {'x', '+', '+', 0};
-    for ( int i = 0; i < 4; i++ ) {
-        long n = 0;
-        const char* q = p;
-        while ( *q >= '0' && *q <= '9' && n < (1L << 30) )
-            n = n * 10 + (*q++ - '0');
-        if ( q == p || n >= (1L << 30) || *q != seps[i] ) return -1;
-        v[i] = (int)n;
-        p = q + 1;
-    }
-    return v[0] >= 1 && v[1] >= 1 ? 0 : -1;
-}
-
 /* [ref: src/gpujpeg_decoder.c:485-531] */
 int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt, const char* val)
 {
@@ -1663,7 +1668,7 @@ int gpujpeg_decoder_set_option(struct gpujpeg_decoder* decoder, const char* opt,
             return GPUJPEG_NOERR;
         }
         int v[4];
-        if ( parse_crop(val, v) ) {
+        if ( gj_parse_crop(val, v) ) {
             GJ_ERR("Invalid crop: %s (WxH+X+Y with W, H >= 1, or none)\n", val);
             return GPUJPEG_ERROR;
         }

@@ -205,6 +205,9 @@ struct gj_orient_map {
 /* value of dec_opt_orientation: "none" -> mode 0, "auto" -> mode 1, "<deg>[-]" (0, 90, 180, 270; '-' = mirrored) -> mode 2 with
  * rot = deg / 90 and flip; 0 on success */
 int gj_parse_orientation(const char* val, int* mode, int* rot, int* flip);
+/* value of dec_opt_crop / tran_opt_crop other than "none": djpeg's -crop syntax "WxH+X+Y", decimal, v = {W, H, X, Y} with W, H >= 1;
+ * 0 on success */
+int gj_parse_crop(const char* val, int v[4]);
 /* The w x h image turned rot quarter turns clockwise, then mirrored horizontally if flip: its size *ow x *oh; the map of the
  * rectangle crop = {x, y, w, h} of it (NULL: all of it) and src = {x, y, w, h}, the rectangle of the w x h image it shows.
  * Returns -1 (and leaves the outputs alone) if crop does not lie inside the oriented image. */
@@ -235,6 +238,15 @@ struct gj_transcode_plan {
 #define GJ_WHY_BYTES 160
 int gj_transcode_plan(int w, int h, int comp_count, const int* hs, const int* vs, int src_interleaved, int out_interleaved, int rot,
                       int flip, int perfect, struct gj_transcode_plan* plan, char* why);
+/* tran_opt_crop (jpegtran -crop with -trim): the plan `full` of a w x h source (gj_transcode_plan's output) cut to the rectangle
+ * rect = {x, y, w, h} of the transformed image.  Refused unless the rectangle lies inside the untrimmed transformed image; its
+ * origin is rounded down to the output's iMCU grid, and refused if that lies in the strip the trim drops; the output reaches to
+ * the rectangle's far edge, clipped to full's output.  Every component's block map is full's, shifted by the origin's blocks,
+ * over the smaller output grid.  Returns 0, or -1 with the reason in why (GJ_WHY_BYTES). */
+int gj_transcode_crop(const struct gj_transcode_plan* full, int w, int h, int comp_count, int out_interleaved, const int rect[4],
+                      struct gj_transcode_plan* plan, char* why);
+/* the source blocks the block maps of plan read (dummy blocks read their clamped neighbours), per component */
+void gj_transcode_window(const struct gj_transcode_plan* plan, int comp_count, struct gj_blk_rect win[GJ_MAX_COMP]);
 /* the COM segments of a JPEG file in front of its first SOS, markers included, copied to out (NULL: size only); their size */
 size_t gj_com_segments(const uint8_t* data, size_t size, uint8_t* out);
 
@@ -718,7 +730,14 @@ struct gj_coef_frame {
     const uint8_t* com;               /* the COM segments in front of the first SOS, markers included */
     size_t com_size;
 };
-int gj_decoder_decode_coefficients(struct gpujpeg_decoder* d, const uint8_t* image, size_t image_size, struct gj_coef_frame* f);
+/* window: NULL, or called once per frame when its geometry g is set (progressive: the block grids the scans decode into) and
+ * before any Huffman decoding, with the stream's metadata read so far.  It returns -1 to refuse the frame, 0 to decode every
+ * block, or 1 to decode only the restart segments that hold the blocks win[c] of every component (gj_crop_pick,
+ * gj_prog_crop_pick); the extents of the blocks left undecoded are 0, so they read as zero. */
+typedef int (*gj_coef_window_fn)(void* ctx, const struct gj_geometry* g, int progressive, const struct gpujpeg_image_metadata* md,
+                                 struct gj_blk_rect win[GJ_MAX_COMP]);
+int gj_decoder_decode_coefficients(struct gpujpeg_decoder* d, const uint8_t* image, size_t image_size, gj_coef_window_fn window,
+                                   void* ctx, struct gj_coef_frame* f);
 
 /* The encoder from coefficients (gj_encoder.c): gj_encoder_setup_coefficients sizes the encoder for a frame of parameters p
  * (RESTART_AUTO as gpujpeg_encoder_encode resolves it for the frame, no segment info) and width x height with the header composed from comp_q / comp_tq, the COM

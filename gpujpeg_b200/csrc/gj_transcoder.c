@@ -4,7 +4,9 @@
  * One decoder and one encoder on the transcoder's stream, so that stream order serialises them:
  *
  *     decoder up to its raw quantised coefficients (K0, K3 or the progressive scans; gj_decoder_decode_coefficients)
- *       -> host plan: trim, output size and sampling, block maps (gj_transcode_plan)
+ *       -> host plan: trim, output size and sampling, block maps (gj_transcode_plan); with tran_opt_crop the plan is cut to the
+ *          rectangle (gj_transcode_crop) inside the decode, once the frame's geometry is known, so that the decoder Huffman-decodes
+ *          only the restart segments that hold the blocks the cut plan reads (gj_transcode_window)
  *       -> k_coef_transform: the decoder's blocks -> the encoder's coefficients and non-zero masks, turned / mirrored, with
  *          the baseline range check (one synchronisation: a frame out of range is refused before anything is written)
  *       -> the encoder's work after K1 (fitted tables, K2, copies; gj_encoder_finish)
@@ -25,6 +27,7 @@ struct gpujpegx_transcoder {
     int mode, rot, flip;   /* tran_opt_transform as gj_parse_orientation gives it: 0 none, 1 auto, 2 rot / flip */
     int perfect;
     int restart;           /* RESTART_AUTO or the interval */
+    int crop, crop_rect[4];   /* tran_opt_crop: set, and x, y, w, h of the transformed image */
     uint32_t* d_range;
     uint32_t* h_range;     /* pinned */
 };
@@ -90,16 +93,90 @@ GPUJPEG_API int gpujpegx_transcoder_set_option(struct gpujpegx_transcoder* t, co
         t->restart = (int)n;
         return 0;
     }
+    if ( strcmp(opt, GPUJPEGX_TRAN_OPT_CROP) == 0 ) {
+        if ( strcmp(val, "none") == 0 ) {
+            t->crop = 0;
+            return 0;
+        }
+        int v[4];
+        if ( gj_parse_crop(val, v) ) {
+            GJ_ERR("Wrong " GPUJPEGX_TRAN_OPT_CROP " value: %s (WxH+X+Y with W, H >= 1, or none)\n", val);
+            return -1;
+        }
+        t->crop = 1;
+        t->crop_rect[0] = v[2];
+        t->crop_rect[1] = v[3];
+        t->crop_rect[2] = v[0];
+        t->crop_rect[3] = v[1];
+        return 0;
+    }
     if ( strcmp(opt, GPUJPEGX_TRAN_OPT_HUFFMAN) == 0 ) return gpujpeg_encoder_set_option(t->enc, GPUJPEG_ENC_OPT_HUFFMAN, val);
     GJ_ERR("Invalid transcoder option: %s!\n", opt);
     return -1;
 }
 
+/* a frame's orientation, output interleaving and plan (cut to tran_opt_crop's rectangle) */
+struct frame_plan {
+    const struct gpujpegx_transcoder* t;
+    int transformed, out_il;
+    struct gj_transcode_plan plan;
+};
+
+static int make_plan(struct frame_plan* fp, const struct gj_geometry* g, int progressive, const struct gpujpeg_image_metadata* md)
+{
+    const struct gpujpegx_transcoder* t = fp->t;
+    const int n = g->comp_count;
+    int rot = t->rot, flip = t->flip;
+    if ( t->mode == 1 ) {
+        const int set = md->vals[GPUJPEG_METADATA_ORIENTATION].set;
+        rot = set ? (int)md->vals[GPUJPEG_METADATA_ORIENTATION].orient.rotation : 0;
+        flip = set ? (int)md->vals[GPUJPEG_METADATA_ORIENTATION].orient.flip : 0;
+    }
+    fp->transformed = t->mode != 0 && (rot != 0 || flip != 0);
+    if ( !fp->transformed ) rot = flip = 0;
+
+    /* the output keeps the source's interleaving; a progressive frame of several components becomes one interleaved scan */
+    fp->out_il = progressive ? n > 1 : g->interleaved;
+    int hs[GJ_MAX_COMP], vs[GJ_MAX_COMP];
+    for ( int c = 0; c < n; c++ ) {
+        hs[c] = g->comp[c].hs;
+        vs[c] = g->comp[c].vs;
+    }
+    char why[GJ_WHY_BYTES];
+    if ( gj_transcode_plan(g->width, g->height, n, hs, vs, g->interleaved, fp->out_il, rot, flip, t->perfect, &fp->plan, why) ) {
+        GJ_ERR("Cannot transcode: %s.\n", why);
+        return -1;
+    }
+    if ( t->crop ) {
+        const struct gj_transcode_plan full = fp->plan;
+        if ( gj_transcode_crop(&full, g->width, g->height, n, fp->out_il, t->crop_rect, &fp->plan, why) ) {
+            GJ_ERR("Cannot transcode: %s.\n", why);
+            return -1;
+        }
+    }
+    return 0;
+}
+
+/* the decoder's window (gj_coef_window_fn) for tran_opt_crop: the plan, and the source blocks it reads */
+static int crop_window(void* ctx, const struct gj_geometry* g, int progressive, const struct gpujpeg_image_metadata* md,
+                       struct gj_blk_rect win[GJ_MAX_COMP])
+{
+    struct frame_plan* fp = (struct frame_plan*)ctx;
+    if ( make_plan(fp, g, progressive, md) ) return -1;
+    gj_transcode_window(&fp->plan, g->comp_count, win);
+    for ( int c = 0; c < g->comp_count; c++ )   /* a window of every block decodes as a frame without one */
+        if ( win[c].bx0 > 0 || win[c].by0 > 0 || win[c].bx1 < g->comp[c].bcx || win[c].by1 < g->comp[c].bcy ) return 1;
+    return 0;
+}
+
 GPUJPEG_API int gpujpegx_transcode(struct gpujpegx_transcoder* t, const uint8_t* jpeg, size_t size, uint8_t** out, size_t* out_size)
 {
     if ( !t || !jpeg || !out || !out_size ) return -1;
+    struct frame_plan fp;
+    memset(&fp, 0, sizeof fp);
+    fp.t = t;
     struct gj_coef_frame f;
-    if ( gj_decoder_decode_coefficients(t->dec, jpeg, size, &f) ) return -1;
+    if ( gj_decoder_decode_coefficients(t->dec, jpeg, size, t->crop ? crop_window : NULL, &fp, &f) ) return -1;
     const struct gj_geometry* g = f.geo;
     const int n = g->comp_count;
     if ( f.color_space != GPUJPEG_YCBCR_BT601_256LVLS &&
@@ -107,28 +184,10 @@ GPUJPEG_API int gpujpegx_transcode(struct gpujpegx_transcoder* t, const uint8_t*
         GJ_ERR("Transcoding a %d-component %s stream is not supported.\n", n, gpujpeg_color_space_get_name(f.color_space));
         return -1;
     }
-    int rot = t->rot, flip = t->flip;
-    if ( t->mode == 1 ) {
-        const int set = f.metadata.vals[GPUJPEG_METADATA_ORIENTATION].set;
-        rot = set ? (int)f.metadata.vals[GPUJPEG_METADATA_ORIENTATION].orient.rotation : 0;
-        flip = set ? (int)f.metadata.vals[GPUJPEG_METADATA_ORIENTATION].orient.flip : 0;
-    }
-    const int transformed = t->mode != 0 && (rot != 0 || flip != 0);
-    if ( !transformed ) rot = flip = 0;
-
-    /* the output keeps the source's interleaving; a progressive frame of several components becomes one interleaved scan */
-    const int out_il = f.progressive ? n > 1 : g->interleaved;
-    int hs[GJ_MAX_COMP], vs[GJ_MAX_COMP];
-    for ( int c = 0; c < n; c++ ) {
-        hs[c] = g->comp[c].hs;
-        vs[c] = g->comp[c].vs;
-    }
-    struct gj_transcode_plan plan;
-    char why[GJ_WHY_BYTES];
-    if ( gj_transcode_plan(g->width, g->height, n, hs, vs, g->interleaved, out_il, rot, flip, t->perfect, &plan, why) ) {
-        GJ_ERR("Cannot transcode: %s.\n", why);
-        return -1;
-    }
+    /* (a cropped frame's plan was made inside the decode, on the metadata its window saw) */
+    if ( !t->crop && make_plan(&fp, g, f.progressive, &f.metadata) ) return -1;
+    const struct gj_transcode_plan plan = fp.plan;
+    const int transformed = fp.transformed, out_il = fp.out_il;
 
     /* quantisation tables: the source's, transposed with the blocks; a table id that two components use with different tables
      * (a progressive frame may redefine one between the components' first scans) moves to a free id */

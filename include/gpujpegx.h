@@ -71,6 +71,19 @@ struct gpujpegx_transcoder;
 #define GPUJPEGX_TRAN_OPT_RESTART "tran_opt_restart"
 /* "standard" (default: T.81 Annex K tables) or "optimized" (tables fitted to the frame, as enc_opt_huffman=optimized) */
 #define GPUJPEGX_TRAN_OPT_HUFFMAN "tran_opt_huffman"
+/* "none" (default) or "WxH+X+Y" (the grammar of dec_opt_crop): jpegtran -crop with -trim, a rectangle of the transformed image
+ * (after tran_opt_transform, so "auto" crops the upright image) rewritten without re-encoding.  With W_u x H_u the transformed
+ * source and W_t x H_t the output without a crop (W_u x H_u trimmed to whole output iMCUs along a reversed axis):
+ *   - refused unless X + W <= W_u and Y + H <= H_u;
+ *   - the origin is rounded down to the output's iMCU grid (8 * max h x 8 * max v samples after the transform): X0, Y0; refused
+ *     if X0 >= W_t or Y0 >= H_t (the rectangle starts in the edge strip the trim drops);
+ *   - the output is (min(X + W, W_t) - X0) x (min(Y + H, H_t) - Y0): the uncropped output's blocks from (X0, Y0) on, whole iMCUs
+ *     of the source's MCU padding included, a block past the source's grid keeping only its clamped neighbour's DC;
+ *   - everything else as without a crop (tables, COM segments, orientation metadata, perfect -- checked on the whole frame --,
+ *     the automatic restart interval for the output's size); only the rectangle's coefficients are range-checked, and only the
+ *     restart segments that hold its blocks are Huffman-decoded;
+ *   - a rectangle of all of W_t x H_t gives the bytes of no crop. */
+#define GPUJPEGX_TRAN_OPT_CROP "tran_opt_crop"
 
 /* NULL without a device */
 GPUJPEG_API struct gpujpegx_transcoder* gpujpegx_transcoder_create(cudaStream_t stream);
