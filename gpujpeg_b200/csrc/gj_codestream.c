@@ -659,6 +659,37 @@ void gj_k4_choose(const struct gj_geometry* g, const struct gj_k4_request* r, st
     p->planes_bytes = p->to_planes ? g->coef_count / 64 * (size_t)(p->n * p->n) : 0;
 }
 
+/* - The flip acts on the component planes, padding included [ref: src/gpujpeg_preprocessor.cu:474-485]: in general only the
+ *   generic pass, which has planes, can do it.  When no component is subsampled vertically and the height has no padding,
+ *   flipping the planes is flipping the image rows, and the fused kernels do that by reading the rows last to first.  (With
+ *   vertical subsampling the two differ: the reference keeps every second row of the UNFLIPPED image -- unlike K4, whose
+ *   fused flip needs only whole MCU rows.)
+ * - enc_opt_writer=libjpeg: libjpeg's fused kernel.  (A flipped frame is planned as any other flipped frame; the encoder refuses
+ *   to encode it.)
+ * - The stripe pipeline feeds the fused kernels rows as they arrive: RGB and libjpeg's colour frames, as stored. */
+void gj_k1_choose(const struct gj_geometry* g, const struct gj_k1_request* r, struct gj_k1_plan* p)
+{
+    memset(p, 0, sizeof *p);
+    p->mcu_rows = (g->bcy + g->max_vs - 1) / g->max_vs;
+    if ( r->coef_input ) return;
+    const int pitch_flip = !r->libjpeg && r->in == GJ_IN_RGB && g->max_vs == 1 && g->height % 8 == 0;
+    const int in = r->flipped && !pitch_flip ? GJ_IN_GENERIC : r->in;
+    const int libjpeg = r->libjpeg && !r->flipped;
+    p->raw_layout = libjpeg || in != GJ_IN_RGB;
+    if ( libjpeg || in == GJ_IN_RGB ) {
+        p->kernel = GJ_K1_FUSED;
+        p->flavour = libjpeg ? GJ_FDCT_ISLOW : 0;
+        p->flip = r->flipped ? GJ_K1_FLIP_PITCH : GJ_K1_FLIP_NONE;
+        p->stripes = !r->flipped && !r->channel_remap && g->comp_count == 3;
+    }
+    else {
+        p->kernel = GJ_K1_BLOCKS;
+        p->convert = in == GJ_IN_GENERIC;
+        p->planes_bytes = p->convert ? g->coef_count : 0;
+        p->flip = r->flipped ? GJ_K1_FLIP_PLANES : GJ_K1_FLIP_NONE;
+    }
+}
+
 /* ------------------------------------------------------------------------------------------- */
 /* writer                                                                                        */
 

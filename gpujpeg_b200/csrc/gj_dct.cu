@@ -1471,71 +1471,6 @@ IdctParams idct_params(const struct gj_dev_dec_tables* h_tables, const int* comp
 
 }  // namespace
 
-/* `bcy` block rows starting at the pointers given; `nblk` = blocks of a whole component plane (the distance between the
- * components' coefficients), so that a frame can be transformed stripe by stripe */
-static int launch_fdct_rgb444(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
-                              int bcx, int bcy, int nblk, const struct gj_dev_enc_tables* h_tables, gj_stream_t stream)
-{
-    FdctParams prm;
-    memcpy(prm.fwd_zz, h_tables->fwd_zz, sizeof prm.fwd_zz);
-    const dim3 grid((bcx + TB - 1) / TB, bcy);
-    /* > 48 KB of dynamic shared memory needs an opt-in, once per device */
-    static int attr_done[64];   // set once per device; two host threads racing write the same value
-    int dev = 0;
-    if ( cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 ) return -1;
-    if ( !__atomic_load_n(&attr_done[dev], __ATOMIC_ACQUIRE) ) {
-        if ( cudaFuncSetAttribute(k_fdct_rgb444<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM) != cudaSuccess ||
-             cudaFuncSetAttribute(k_fdct_rgb444<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM) != cudaSuccess )
-            return -1;
-        __atomic_store_n(&attr_done[dev], 1, __ATOMIC_RELEASE);
-    }
-    /* Two ways of getting the pixels on chip: plain coalesced loads, or copy-engine bulk copies into a persistent CTA
-     * (profiles/k1_times.py times both).  The kernel is bound by instruction issue, not by the loads, and the bulk variant
-     * pays two CTA-wide barriers per strip at 3 instead of 4 CTAs per SM.  The plain-load kernel is the default;
-     * GPUJPEG_B200_K1=bulk selects the other one (rows must be 16-byte aligned). */
-    static int use_bulk = -1;
-    if ( use_bulk < 0 ) {
-        const char* e = getenv("GPUJPEG_B200_K1");
-        use_bulk = e && strcmp(e, "bulk") == 0;
-    }
-    const bool aligned16 = ((reinterpret_cast<uintptr_t>(d_raw) | (size_t)pitch) & 15) == 0 && ((size_t)(width % STRIP_PX) * 3) % 16 == 0;
-    if ( use_bulk && aligned16 ) {
-        static int bulk_attr[64];
-        if ( !__atomic_load_n(&bulk_attr[dev], __ATOMIC_ACQUIRE) ) {
-            if ( cudaFuncSetAttribute(k_fdct_rgb444_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, K1T_SMEM) != cudaSuccess ) return -1;
-            __atomic_store_n(&bulk_attr[dev], 1, __ATOMIC_RELEASE);
-        }
-        int sms = 132;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        const int n_strips = (int)grid.x * (int)grid.y;
-        const int ctas = n_strips < sms * 3 ? n_strips : sms * 3;   // 3 CTAs of 64.5 KB per SM
-        k_fdct_rgb444_bulk<<<ctas, NT, K1T_SMEM, stream>>>(d_raw, width, height, (size_t)pitch, d_coef, d_nzmask, bcx, bcy, nblk, prm);
-    }
-    else if ( pick_vec(d_raw, (size_t)pitch) == 4 )
-        gj_launch_pdl(k_fdct_rgb444<4>, grid, dim3(NT), K1_SMEM, stream, d_raw, width, height, (size_t)pitch, d_coef, d_nzmask, bcx, nblk, prm);
-    else
-        gj_launch_pdl(k_fdct_rgb444<1>, grid, dim3(NT), K1_SMEM, stream, d_raw, width, height, (size_t)pitch, d_coef, d_nzmask, bcx, nblk, prm);
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
-}
-
-extern "C" int gj_launch_fdct_rgb444(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef,
-                                     uint64_t* d_nzmask, int bcx, int bcy, const struct gj_dev_enc_tables* h_tables,
-                                     gj_stream_t stream)
-{
-    return launch_fdct_rgb444(d_raw, width, height, pitch, d_coef, d_nzmask, bcx, bcy, bcx * bcy, h_tables, stream);
-}
-/* block rows [by0, by1) of the frame only (the encoder's stripe pipeline: rows are transformed while later rows still arrive) */
-extern "C" int gj_launch_fdct_rgb444_rows(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef,
-                                          uint64_t* d_nzmask, int bcx, int bcy, int by0, int by1,
-                                          const struct gj_dev_enc_tables* h_tables, gj_stream_t stream)
-{
-    if ( by0 < 0 || by1 > bcy || by0 >= by1 ) return -1;
-    const int rows = (by1 * 8 < height ? by1 * 8 : height) - by0 * 8;
-    return launch_fdct_rgb444(d_raw + (ptrdiff_t)by0 * 8 * pitch, width, rows, pitch, d_coef + (size_t)by0 * bcx * 64,
-                              d_nzmask + (size_t)by0 * bcx, bcx, by1 - by0, bcx * bcy, h_tables, stream);
-}
-
-/* ---- subsampled variants: luminance hs x vs in {2x1, 2x2, 1x2}, chrominance 1x1 ---- */
 /* The block grids of the three components restricted to the MCU rows [my0, my1) (an MCU row = 8 * vs image rows): the kernels
  * index every plane from its first block of the range, so a frame can be transformed stripe by stripe.  Returns the image
  * rows the range holds. */
@@ -1553,116 +1488,6 @@ static int ss_grid_rows(SsGrid* sg, const struct gj_comp_geo comp[3], int my0, i
     return y1 > y0 ? y1 - y0 : 0;
 }
 
-extern "C" int gj_launch_fdct_rgb_ss_rows(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef,
-                                          uint64_t* d_nzmask, const struct gj_comp_geo comp[3], int my0, int my1,
-                                          const struct gj_dev_enc_tables* h_tables, gj_stream_t stream)
-{
-    FdctParams prm;
-    memcpy(prm.fwd_zz, h_tables->fwd_zz, sizeof prm.fwd_zz);
-    const int hs = comp[0].hs, vs = comp[0].vs;
-    if ( comp[1].hs != 1 || comp[1].vs != 1 || comp[2].hs != 1 || comp[2].vs != 1 ) return -1;
-    const int mcu_rows = (comp[0].bcy + vs - 1) / vs;
-    if ( my0 < 0 || my1 > mcu_rows || my0 >= my1 ) return -1;
-    SsGrid sg;
-    height = ss_grid_rows(&sg, comp, my0, my1, height);
-    d_raw += (ptrdiff_t)my0 * 8 * vs * pitch;
-    const dim3 grid((comp[0].bcx + TB - 1) / TB, my1 - my0);
-    const int vec = pick_vec(d_raw, (size_t)pitch);
-    static int attr_done[64][4];   // the shared-memory opt-in of a template instance, once per device
-    int dev = 0;
-    if ( cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 ) return -1;
-#define GJ_K1SS(H, V)                                                                                                        \
-    do {                                                                                                                     \
-        constexpr int nt = TB * V + 2 * TB / H;                                                                              \
-        constexpr int sm = nt * BLK_F * 4;                                                                                   \
-        if ( !__atomic_load_n(&attr_done[dev][H * 2 + V - 3], __ATOMIC_ACQUIRE) ) {                                          \
-            if ( cudaFuncSetAttribute(k_fdct_rgb_ss<H, V, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm) != cudaSuccess || \
-                 cudaFuncSetAttribute(k_fdct_rgb_ss<H, V, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, sm) != cudaSuccess )  \
-                return -1;                                                                                                   \
-            __atomic_store_n(&attr_done[dev][H * 2 + V - 3], 1, __ATOMIC_RELEASE);                                           \
-        }                                                                                                                    \
-        if ( vec == 4 )                                                                                                      \
-            gj_launch_pdl(k_fdct_rgb_ss<H, V, 4>, grid, dim3(nt), sm, stream, d_raw, width, height, (size_t)pitch, d_coef, d_nzmask, sg, prm); \
-        else                                                                                                                 \
-            gj_launch_pdl(k_fdct_rgb_ss<H, V, 1>, grid, dim3(nt), sm, stream, d_raw, width, height, (size_t)pitch, d_coef, d_nzmask, sg, prm); \
-    } while ( 0 )
-    if ( hs == 2 && vs == 2 ) GJ_K1SS(2, 2);
-    else if ( hs == 2 && vs == 1 ) GJ_K1SS(2, 1);
-    else if ( hs == 1 && vs == 2 ) GJ_K1SS(1, 2);
-    else return -1;
-#undef GJ_K1SS
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
-}
-extern "C" int gj_launch_fdct_rgb_ss(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef,
-                                     uint64_t* d_nzmask, const struct gj_comp_geo comp[3],
-                                     const struct gj_dev_enc_tables* h_tables, gj_stream_t stream)
-{
-    const int vs = comp[0].vs > 0 ? comp[0].vs : 1;
-    return gj_launch_fdct_rgb_ss_rows(d_raw, width, height, pitch, d_coef, d_nzmask, comp, 0, (comp[0].bcy + vs - 1) / vs, h_tables,
-                                      stream);
-}
-
-/* ---- enc_opt_writer=libjpeg ---- */
-extern "C" int gj_launch_fdct_libjpeg_rows(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
-                                           const struct gj_comp_geo* comp, int comp_count, int my0, int my1, const uint8_t raw_q[2][64],
-                                           gj_stream_t stream)
-{
-    const int hs = comp[0].hs, vs = comp[0].vs;
-    if ( comp_count != 1 && comp_count != 3 ) return -1;
-    if ( comp_count == 3 && (comp[1].hs != 1 || comp[1].vs != 1 || comp[2].hs != 1 || comp[2].vs != 1) ) return -1;
-    if ( comp_count == 1 && (hs != 1 || vs != 1) ) return -1;
-    const int mcu_rows = (comp[0].bcy + vs - 1) / vs;
-    if ( my0 < 0 || my1 > mcu_rows || my0 >= my1 ) return -1;
-    LjGrid lg;
-    memset(&lg, 0, sizeof lg);
-    for ( int c = 0; c < comp_count; c++ ) {
-        const int per = c == 0 ? vs : 1;   /* block rows of the component per MCU row */
-        const int lo = my0 * per, hi = my1 * per < comp[c].bcy ? my1 * per : comp[c].bcy;
-        lg.bcx[c] = comp[c].bcx;
-        lg.bcy[c] = hi > lo ? hi - lo : 0;
-        lg.blk_off[c] = comp[c].blk_off + lo * comp[c].bcx;
-        lg.wib[c] = (comp[c].width + 7) / 8;
-        lg.hib[c] = (comp[c].height + 7) / 8 - lo;
-    }
-    const int y0 = my0 * 8 * vs, y1 = my1 * 8 * vs < height ? my1 * 8 * vs : height;
-    height = y1 - y0;
-    d_raw += (ptrdiff_t)y0 * pitch;
-    LjParams prm;
-    for ( int t = 0; t < 2; t++ )
-        for ( int k = 0; k < 64; k++ ) {
-            prm.q[t][k] = raw_q[t][k];
-            prm.recip[t][k] = gj_quant_recip_libjpeg(raw_q[t][k]);
-        }
-    const dim3 grid((comp[0].bcx + TB - 1) / TB, my1 - my0);
-    const int vec = pick_vec(d_raw, (size_t)pitch);
-#define GJ_K1LJ(H, V, N)                                                                                                         \
-    do {                                                                                                                         \
-        using S = LjShape<H, V, N>;                                                                                              \
-        if ( vec == 4 )                                                                                                          \
-            gj_launch_pdl(k_fdct_libjpeg<H, V, N, 4>, grid, dim3(S::NTS), S::SMEM, stream, d_raw, width, height, (size_t)pitch, d_coef, \
-                          d_nzmask, lg, prm);                                                                                    \
-        else                                                                                                                     \
-            gj_launch_pdl(k_fdct_libjpeg<H, V, N, 1>, grid, dim3(S::NTS), S::SMEM, stream, d_raw, width, height, (size_t)pitch, d_coef, \
-                          d_nzmask, lg, prm);                                                                                    \
-    } while ( 0 )
-    if ( comp_count == 1 ) GJ_K1LJ(1, 1, 1);
-    else if ( hs == 1 && vs == 1 ) GJ_K1LJ(1, 1, 3);
-    else if ( hs == 2 && vs == 1 ) GJ_K1LJ(2, 1, 3);
-    else if ( hs == 2 && vs == 2 ) GJ_K1LJ(2, 2, 3);
-    else if ( hs == 1 && vs == 2 ) GJ_K1LJ(1, 2, 3);
-    else return -1;
-#undef GJ_K1LJ
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
-}
-extern "C" int gj_launch_fdct_libjpeg(const uint8_t* d_raw, int width, int height, int pitch, int16_t* d_coef, uint64_t* d_nzmask,
-                                      const struct gj_comp_geo* comp, int comp_count, const uint8_t raw_q[2][64], gj_stream_t stream)
-{
-    const int vs = comp[0].vs > 0 ? comp[0].vs : 1;
-    return gj_launch_fdct_libjpeg_rows(d_raw, width, height, pitch, d_coef, d_nzmask, comp, comp_count, 0, (comp[0].bcy + vs - 1) / vs,
-                                       raw_q, stream);
-}
-
-/* ---- no colour transform: grey, planar and packed YCbCr formats ---- */
 static int sample_grid(SampleGrid* sg, const struct gj_raw_layout* raw, const struct gj_comp_geo* comp, int comp_count,
                        const uint8_t* comp_tbl)
 {
@@ -1688,16 +1513,117 @@ static int sample_grid(SampleGrid* sg, const struct gj_raw_layout* raw, const st
     return total;
 }
 
-extern "C" int gj_launch_fdct_samples(const uint8_t* d_raw, const struct gj_raw_layout* raw, int16_t* d_coef,
-                                      uint64_t* d_nzmask, const struct gj_comp_geo* comp, int comp_count,
-                                      const uint8_t* comp_tbl, const struct gj_dev_enc_tables* h_tables, gj_stream_t stream)
+/* > 48 KB of dynamic shared memory needs an opt-in: once per kernel and device (two host threads racing write the same value) */
+template <auto K>
+static int smem_opt_in(int smem, int dev)
 {
+    static int done[64];
+    if ( __atomic_load_n(&done[dev], __ATOMIC_ACQUIRE) ) return 0;
+    if ( cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ) return -1;
+    __atomic_store_n(&done[dev], 1, __ATOMIC_RELEASE);
+    return 0;
+}
+
+extern "C" int gj_launch_fdct_fused(const struct gj_k1_plan* p, const struct gj_geometry* g, const uint8_t* d_raw, int pitch, int my0,
+                                    int my1, const struct gj_dev_enc_tables* h_tables, const uint8_t raw_q[2][64], int16_t* d_coef,
+                                    uint64_t* d_nzmask, gj_stream_t stream)
+{
+    const struct gj_comp_geo* comp = g->comp;
+    const int hs = comp[0].hs, vs = comp[0].vs;
+    if ( g->comp_count == 3 && (comp[1].hs != 1 || comp[1].vs != 1 || comp[2].hs != 1 || comp[2].vs != 1) ) return -1;
+    if ( my0 < 0 || my1 > p->mcu_rows || my0 >= my1 ) return -1;
+    int dev = 0;
+    if ( cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 ) return -1;
+    if ( p->flip == GJ_K1_FLIP_PITCH ) {   /* enc_opt_flipped: rows are read last to first */
+        d_raw += (size_t)(g->height - 1) * (size_t)pitch;
+        pitch = -pitch;
+    }
+    /* the rows and planes from the range's first MCU row on, so that a frame can be transformed stripe by stripe */
+    SsGrid sg;
+    const int rows = ss_grid_rows(&sg, comp, my0, my1, g->height);
+    d_raw += (ptrdiff_t)my0 * 8 * vs * pitch;
+    const dim3 grid((comp[0].bcx + TB - 1) / TB, my1 - my0);
+    /* Two ways of getting the 4:4:4 pixels on chip: plain coalesced loads, or copy-engine bulk copies into a persistent CTA
+     * (profiles/k1_times.py times both).  The kernel is bound by instruction issue, not by the loads, and the bulk variant
+     * pays two CTA-wide barriers per strip at 3 instead of 4 CTAs per SM.  The plain-load kernel is the default;
+     * GPUJPEG_B200_K1=bulk selects the other one (rows must be 16-byte aligned). */
+    static int use_bulk = -1;
+    if ( use_bulk < 0 ) {
+        const char* e = getenv("GPUJPEG_B200_K1");
+        use_bulk = e && strcmp(e, "bulk") == 0;
+    }
+    const bool aligned16 = ((reinterpret_cast<uintptr_t>(d_raw) | (size_t)pitch) & 15) == 0 && ((size_t)(g->width % STRIP_PX) * 3) % 16 == 0;
+    auto launch = [&](auto H, auto V, auto VEC, auto F, auto NC) {
+        /* the instances: libjpeg's flavour on RGB and on grey (4:4:4 only), this library's on RGB */
+        if constexpr ( F == GJ_FDCT_ISLOW && (NC == 3 || (H == 1 && V == 1)) ) {
+            using S = LjShape<H, V, NC>;
+            LjGrid lg;
+            memset(&lg, 0, sizeof lg);
+            for ( int c = 0; c < NC; c++ ) {
+                lg.bcx[c] = sg.bcx[c];
+                lg.bcy[c] = sg.bcy[c];
+                lg.blk_off[c] = sg.blk_off[c];
+                lg.wib[c] = (comp[c].width + 7) / 8;
+                lg.hib[c] = (comp[c].height + 7) / 8 - my0 * (c == 0 ? V : 1);
+            }
+            LjParams prm;
+            for ( int t = 0; t < 2; t++ )
+                for ( int k = 0; k < 64; k++ ) {
+                    prm.q[t][k] = raw_q[t][k];
+                    prm.recip[t][k] = gj_quant_recip_libjpeg(raw_q[t][k]);
+                }
+            gj_launch_pdl(k_fdct_libjpeg<H, V, NC, VEC>, grid, dim3(S::NTS), S::SMEM, stream, d_raw, g->width, rows, (size_t)pitch, d_coef,
+                          d_nzmask, lg, prm);
+            return 0;
+        }
+        else if constexpr ( F == 0 && NC == 3 ) {
+            FdctParams prm;
+            memcpy(prm.fwd_zz, h_tables->fwd_zz, sizeof prm.fwd_zz);
+            if constexpr ( H == 1 && V == 1 ) {
+                const int bcx = comp[0].bcx;
+                int16_t* coef = d_coef + (size_t)my0 * bcx * 64;
+                uint64_t* nzmask = d_nzmask + (size_t)my0 * bcx;
+                if ( use_bulk && aligned16 ) {
+                    if ( smem_opt_in<k_fdct_rgb444_bulk>(K1T_SMEM, dev) ) return -1;
+                    int sms = 132;
+                    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+                    const int n_strips = (int)grid.x * (int)grid.y;
+                    const int ctas = n_strips < sms * 3 ? n_strips : sms * 3;   // 3 CTAs of 64.5 KB per SM
+                    k_fdct_rgb444_bulk<<<ctas, NT, K1T_SMEM, stream>>>(d_raw, g->width, rows, (size_t)pitch, coef, nzmask, bcx, my1 - my0,
+                                                                       comp[0].nblk, prm);
+                    return 0;
+                }
+                if ( smem_opt_in<k_fdct_rgb444<VEC>>(K1_SMEM, dev) ) return -1;
+                gj_launch_pdl(k_fdct_rgb444<VEC>, grid, dim3(NT), K1_SMEM, stream, d_raw, g->width, rows, (size_t)pitch, coef, nzmask, bcx,
+                              comp[0].nblk, prm);
+            }
+            else {
+                constexpr int nt = TB * V + 2 * TB / H, smem = nt * BLK_F * 4;
+                if ( smem_opt_in<k_fdct_rgb_ss<H, V, VEC>>(smem, dev) ) return -1;
+                gj_launch_pdl(k_fdct_rgb_ss<H, V, VEC>, grid, dim3(nt), smem, stream, d_raw, g->width, rows, (size_t)pitch, d_coef, d_nzmask,
+                              sg, prm);
+            }
+            return 0;
+        }
+        return -1;
+    };
+    if ( instance(launch, std::tuple<>{}, OneOf<1, 2>{hs}, OneOf<1, 2>{vs}, OneOf<4, 1>{pick_vec(d_raw, (size_t)pitch)},
+                  OneOf<0, GJ_FDCT_ISLOW>{p->flavour}, OneOf<1, 3>{g->comp_count}) )
+        return -1;
+    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+extern "C" int gj_launch_fdct_blocks(const struct gj_k1_plan* p, const uint8_t* d_src, const struct gj_raw_layout* raw,
+                                     const struct gj_comp_geo* comp, int comp_count, const uint8_t* comp_tbl,
+                                     const struct gj_dev_enc_tables* h_tables, int16_t* d_coef, uint64_t* d_nzmask, gj_stream_t stream)
+{
+    if ( p->kernel != GJ_K1_BLOCKS ) return -1;
     FdctParams prm;
     memcpy(prm.fwd_zz, h_tables->fwd_zz, sizeof prm.fwd_zz);
     SampleGrid sg;
     const int total = sample_grid(&sg, raw, comp, comp_count, comp_tbl);
     if ( total <= 0 ) return -1;
-    k_fdct_samples<<<(total + SG_THREADS - 1) / SG_THREADS, SG_THREADS, 0, stream>>>(d_raw, sg, total, d_coef, d_nzmask, prm);
+    k_fdct_samples<<<(total + SG_THREADS - 1) / SG_THREADS, SG_THREADS, 0, stream>>>(d_src, sg, total, d_coef, d_nzmask, prm);
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
