@@ -205,7 +205,10 @@ int gj_geometry_init(struct gj_geometry* g, const struct gpujpeg_parameters* par
         struct gj_raw_layout rl;
         g->raw_size = gj_raw_layout_init(&rl, pi) == 0 ? rl.size : (size_t)g->pitch * pi->height;
     }
-    /* worst case per 8x8 block: 64 x (16-bit code + 11 value bits) < 208 bytes, doubled by stuffing */
+    /* worst case per 8x8 block: a DC code of at most 16 bits + 11 value bits and 63 AC codes of at most 16 + 10 bits, 27 +
+     * 63 x 26 = 1665 bits (209 bytes) before stuffing.  The slots assume that a block's stuffed bytes stay within 416 (2 x 208:
+     * no Huffman code is all 1-bits, so not every byte is 0xFF; tests/test_k2_families.py measures the densest blocks).  K2
+     * never writes past a slot: a segment that needs more is reported (info[1] bit 1) and the frame fails. */
     g->slot_stride = ((size_t)g->seg_mcu * (g->interleaved ? l->bpm : 1) * 416 + 2 + 127) / 128 * 128;
     /* the reference's output budget [ref: src/gpujpeg_writer.c:63-89], 2 bytes per pixel and component -- or per coded
      * sample where padding to whole blocks and MCUs outweighs the image: a frame 1 pixel thin codes 8 rows per real one */

@@ -577,6 +577,27 @@ static struct gj_k1_request k1_request(const struct gpujpeg_encoder* e, int in)
     return r;
 }
 
+/* the host output buffer: at least `size` bytes, pinned or not as asked */
+static int reserve_out(struct gpujpeg_encoder* e, size_t size)
+{
+    if ( e->out_size >= size && e->out_is_pinned == e->out_pinned ) return 0;
+    if ( e->out ) {
+        if ( e->out_is_pinned ) gj_cuda_free_host(e->out);
+        else free(e->out);
+    }
+    e->out = NULL;
+    e->out_size = 0;
+    e->out_is_pinned = e->out_pinned;
+    if ( e->out_pinned ) {
+        if ( gj_cuda_malloc_host((void**)&e->out, size) ) return -1;
+    }
+    else if ( !(e->out = (uint8_t*)malloc(size)) ) {
+        return -1;
+    }
+    e->out_size = size;
+    return 0;
+}
+
 /* (re)build everything that depends on geometry [ref: src/gpujpeg_common.c:628-1106] */
 static int encoder_init_image(struct gpujpeg_encoder* e, const struct gpujpeg_parameters* p,
                               const struct gpujpeg_image_parameters* pi, const struct gj_k1_request* k1)
@@ -620,22 +641,7 @@ static int encoder_init_image(struct gpujpeg_encoder* e, const struct gpujpeg_pa
             return -1;
         e->seg_alloc = g->seg_count;
     }
-    if ( e->out_size < g->stream_cap || e->out_is_pinned != e->out_pinned ) {
-        if ( e->out ) {
-            if ( e->out_is_pinned ) gj_cuda_free_host(e->out);
-            else free(e->out);
-        }
-        e->out = NULL;
-        e->out_size = 0;
-        e->out_is_pinned = e->out_pinned;
-        if ( e->out_pinned ) {
-            if ( gj_cuda_malloc_host((void**)&e->out, g->stream_cap) ) return -1;
-        }
-        else if ( !(e->out = (uint8_t*)malloc(g->stream_cap)) ) {
-            return -1;
-        }
-        e->out_size = g->stream_cap;
-    }
+    if ( reserve_out(e, g->stream_cap) ) return -1;
     e->param = *p;
     e->param_image = *pi;
     e->initialised = 1;
@@ -879,6 +885,25 @@ static int encode_tail(struct gpujpeg_encoder* e, int k2_done, int stats, uint8_
             GJ_ERR("Encoder device allocation failed (%zu bytes): %s\n", (size_t)g->seg_count * e->slot_stride, gj_cuda_last_error());
             return -1;
         }
+        if ( launch_k2(e) || gj_cuda_memcpy_d2h_async(e->h_info, e->d_info_cur, 32, e->stream) ||
+             gj_cuda_stream_sync(e->stream) ) {
+            GJ_ERR("Encoder failed: %s\n", gj_cuda_last_error());
+            return -1;
+        }
+    }
+    if ( e->h_info[1] == 1 && e->h_info[0] > g->stream_cap ) {
+        /* the finished stream outgrew the reference's budget of 2 bytes per sample (K2 counted it all, h_info[0]): a legal
+         * frame can code to more -- a transcoded stream of blocks with 63 AC coefficients at +-1023 takes about 207 bytes per
+         * block, and the worst 8-bit pixel blocks at q100 with short restart intervals exceed 128 bytes per block too.  Grow
+         * the device stream and the host output buffer to that size and run K2 again; the size stays for the encoder's
+         * later frames of this geometry, as the slot size above does. */
+        const size_t need = ((size_t)e->h_info[0] + 4095) / 4096 * 4096;
+        GJ_VERBOSE(e->param.verbose, "Enlarging the stream buffer to %zu bytes.\n", need);
+        if ( grow((void**)&e->d_stream, &e->d_stream_size, need + 64) || reserve_out(e, need) ) {
+            GJ_ERR("Encoder allocation failed (%zu bytes): %s\n", need, gj_cuda_last_error());
+            return -1;
+        }
+        e->geo.stream_cap = need;
         if ( launch_k2(e) || gj_cuda_memcpy_d2h_async(e->h_info, e->d_info_cur, 32, e->stream) ||
              gj_cuda_stream_sync(e->stream) ) {
             GJ_ERR("Encoder failed: %s\n", gj_cuda_last_error());
